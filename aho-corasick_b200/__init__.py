@@ -4,7 +4,7 @@ The names, argument meaning and error behaviour follow BurntSushi/aho-corasick 1
 (`AhoCorasick`, `AhoCorasickBuilder`, `MatchKind`, `StartKind`, `AhoCorasickKind`, `Match`,
 `find_iter`, `find_overlapping_iter`, `try_*`; src/ahocorasick.rs, src/lib.rs:239-251), so the
 parity tests read like the reference's own.  Everything that touches a haystack goes through the
-C ABI (include/acb200.h) into hand-written sm_100a kernels; there is no CPU search path here.
+C ABI (include/acb200.h) into hand-written sm_90a kernels; there is no CPU search path here.
 Python is test/bench glue only: the product is the shared library.
 """
 from __future__ import annotations
@@ -27,7 +27,7 @@ def _load():
     if not _LIB_PATH.exists():
         raise NativeLibraryMissing(
             f"{_LIB_PATH} is missing: build it with `python aho-corasick_b200/build.py` "
-            "(nvcc, sm_100a). There is no fallback implementation.")
+            "(nvcc, sm_90a). There is no fallback implementation.")
     return C.CDLL(str(_LIB_PATH))
 
 

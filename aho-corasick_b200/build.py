@@ -1,4 +1,4 @@
-"""In-tree build of libacb200.so (hand-written sm_100a CUDA + C++ host) with nvcc."""
+"""In-tree build of libacb200.so (hand-written sm_90a CUDA + C++ host) with nvcc."""
 import os
 import shutil
 import subprocess
@@ -9,8 +9,9 @@ CSRC = HERE / "csrc"
 LIB = HERE / "libacb200.so"
 SOURCES = ["acb_build.cpp", "acb_kernels.cu", "acb_prefilter.cu", "acb_comm.cu", "acb_api.cu"]
 HEADERS = ["acb_build.hpp", "acb_comm.hpp", "acb_device.cuh", "acb_ptx.cuh", "../../include/acb200.h", "../../include/acb200_debug.h"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    *GENCODE, "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall", "-shared", "--expt-relaxed-constexpr",
 ]
 
@@ -26,7 +27,8 @@ def needs_build():
     if not LIB.exists():
         return True
     t = LIB.stat().st_mtime
-    return any((CSRC / s).stat().st_mtime > t for s in SOURCES + HEADERS)
+    # this script counts as a source: a library built with other flags (another architecture) is stale
+    return any((CSRC / s).stat().st_mtime > t for s in SOURCES + HEADERS + ["../build.py"])
 
 
 def build_library(force=False, verbose=False):

@@ -485,7 +485,7 @@ void derive_metadata(acg_dfa* a) {
       // the byte from the fingerprint's own low bits.  A multiplicative hash of such short keys is
       // sensitive to the constant, so pick the candidate that lets through the fewest fingerprints
       // drawn from the bytes the patterns use at each position.
-      // First-stage keys.  ACG_EXP_KEY24: the 3-byte fingerprints.  Default (r02 A/B: -2 % cfg 2, -18 % cfg 3): 27-bit keys
+      // First-stage keys.  ACG_EXP_KEY24: the 3-byte fingerprints.  Default (faster on cfg 2 and cfg 3): 27-bit keys
       // -- the 3 bytes plus the low 3 bits of the window's fourth byte, which a shift of 5 instead
       // of 8 in the multiplier keeps at no cost in the kernel.  For a pattern that starts at the
       // probed (even) offset the fourth byte is its own fourth byte; for one that starts one byte
@@ -585,9 +585,9 @@ void derive_metadata(acg_dfa* a) {
   if (h.prefilter_kind == ACG_PRE_START_BYTES || h.prefilter_kind == ACG_PRE_RARE_BYTES) {
     if (h.pre_n) {
       // Needles with offsets (rare bytes in the middle of patterns) turn every occurrence into
-      // back + 1 start offsets to verify; measured on BASELINE config 1's automaton over uniform
-      // printable text (r02f: 4.7 ms against 2.1 ms per 4 GiB for the fingerprint filter), so the scan
-      // is reserved for needles that mark a pattern's first byte.
+      // back + 1 start offsets to verify; on BASELINE config 1's automaton over uniform printable text
+      // that is slower than the fingerprint filter, so the scan is reserved for needles that mark a
+      // pattern's first byte.
       bool ok = true;
       for (uint32_t i = 0; i < h.pre_n; ++i) ok = ok && h.pre_back[i] == 0;
       if (ok) {
@@ -799,7 +799,7 @@ int run_walk_overlapping(const acg_dfa* a, const uint8_t* d_hay, uint64_t readab
   const uint64_t n_bytes = span_end - span_start;
   if (a->max_list_len >= (1u << acb::kTieBits)) return ACG_E_INVALID_ARG;
   if (n_bytes >= (1ull << (64 - acb::kTieBits))) return ACG_E_INVALID_ARG;
-  int dev_sms = 148;
+  int dev_sms = 132;
   cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, a->device);
   const uint64_t target_lanes = uint64_t(dev_sms) * 2048;
   uint64_t seg_len = (n_bytes + target_lanes - 1) / std::max<uint64_t>(target_lanes, 1);
@@ -943,7 +943,7 @@ int order_tuples(const acg_dfa* a, uint64_t want, uint64_t n_bytes, TupleResult*
 
 // ---- pageable host haystacks ---------------------------------------------------------------------
 // cudaMemcpyAsync from pageable memory is staged by the driver through its own page-locked buffers by
-// a single thread (~10 GiB/s on the bench box against 49 GiB/s from pinned memory).  A caller that
+// a single thread, several times slower than a copy from pinned memory.  A caller that
 // hands over an ordinary allocation (a Rust Vec<u8>, a numpy array) gets the same pipeline with the
 // staging done here: host threads copy each chunk into a page-locked ring buffer while the previous
 // chunk is on its way over PCIe.
@@ -1051,7 +1051,7 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
   Workspace& w = cur_ws();
   const uint64_t n_bytes = span_end - span_start;
   if (n_bytes >= (1ull << (64 - acb::kTieBits))) return ACG_E_INVALID_ARG;
-  int dev_sms = 148;
+  int dev_sms = 132;
   cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, a->device);
   // one tuple per 256 haystack bytes to start with (the BASELINE workloads have one per 4 KiB);
   // denser outputs are detected through the counter and the scan is repeated with room

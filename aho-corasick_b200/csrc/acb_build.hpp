@@ -1,4 +1,4 @@
-// acb_build.hpp -- host-side automaton construction for the B200 search path.
+// acb_build.hpp -- host-side automaton construction for the GPU search path.
 //
 // Produces the dense DFA the device kernels consume, with tables that are
 // bit-identical to what the reference's own builder produces for the same

@@ -1,4 +1,4 @@
-// acb_kernels.cu -- sm_100a kernels of the Aho-Corasick search path.
+// acb_kernels.cu -- sm_90a kernels of the Aho-Corasick search path.
 //
 //   K1  walk_overlapping_kernel   sharded DFA state-transition scan; replaces the
 //                                 loop of try_find_overlapping_fwd_imp
@@ -52,13 +52,11 @@ constexpr int kWalkThreads = 256;
 // max_pattern_len-1 bytes before its shard -- the Aho-Corasick state depends on
 // at most that many trailing bytes -- and only reports matches whose end lies
 // inside its shard, so every end offset is owned by exactly one lane.
-// The loop is one dependent table load per byte.  Everything below the first two trie levels (42 % of
-// the transitions on cfg 2) is an L2 hit, one 32-byte sector per byte: at 2.75 ms per GiB the kernel
-// moves 5.2 TB/s of sectors out of L2, which is where random-sector traffic saturates on this part
-// -- more loads in flight do not help.  Measured in r02 and gone (profiles/r02a_ab_walk.jsonl,
-// r02e_walk_cfg2.jsonl, r02f_walk2.jsonl): the start / depth-1 rows staged in shared memory behind a
-// flagged table copy (4.68 ms per GiB), and four independent shards per lane with speculative
-// 16-byte blocks (3.46-3.73 ms per GiB; ncu: long-scoreboard stalls unchanged at 23 per issue).
+// The loop is one dependent table load per byte.  Everything below the first two trie levels is an
+// L2 hit, one 32-byte sector per byte, so the kernel is bound by random-sector traffic out of L2 and
+// more loads in flight do not help.  Tried and dropped as slower: the start / depth-1 rows staged in
+// shared memory behind a flagged table copy, and four independent shards per lane with speculative
+// 16-byte blocks.
 __global__ void __launch_bounds__(kWalkThreads, 5)
 walk_overlapping_kernel(DfaDev d, WalkLaunch p) {
   __shared__ uint8_t s_cls[256];

@@ -1,7 +1,7 @@
 // acb_prefilter.cu -- K3/K3b: position-parallel k-gram prefilter fused with the
 // anchored DFA verify, and the non-overlapping chain resolution.
 //
-// Why this shape on B200: the reference's per-byte loop (src/automaton.rs:1310-1418,
+// Why this shape on a GPU: the reference's per-byte loop (src/automaton.rs:1310-1418,
 // 1491-1534) is one dependent table load per haystack byte -- latency bound, and
 // on a GPU it forces one lane per shard with strided haystack reads.  Testing
 // every *start position* independently instead reads the haystack exactly once,
@@ -33,8 +33,8 @@ namespace {
 // probes), 16 KiB bitmap, two CTAs per SM -- the per-step bookkeeping is spread over twice as many
 // positions, which pays when first-stage hits are rare (few patterns); with frequent hits the 32
 // resident warps of the narrow geometry hide the latency of the second stage and the verifier
-// better.  (A third geometry -- the 2 KiB tile with the 128 KiB bitmap, 20 warps -- was measured in
-// r02 and lost to the narrow one on cfg 2 and cfg 3: profiles/r02a_ab_*.jsonl.)
+// better.  (A third geometry -- the 2 KiB tile with the 128 KiB bitmap, 20 warps -- lost to the
+// narrow one on cfg 2 and cfg 3 and was dropped.)
 enum : int { kGeomNarrow = 0, kGeomWide = 1 };
 template <int GEOM> struct PfGeom {
   static constexpr int kThreads = GEOM == kGeomNarrow ? 1024 : 512;
@@ -230,22 +230,21 @@ __device__ __forceinline__ bool bloom_test(const uint32_t* s_bitmap, uint32_t h)
 // one / two more Bloom hashes of the 4-byte fingerprint in the shared-memory bitmap.  DENSE: looked up
 // in the anchor map (exact: one L2 access tells whether the k bytes begin a pattern and at which
 // trie state), two items per lane in flight.
-// (Measured in r02 and gone: a lane-local second stage without compaction, a paired one, and the
-// anchor-map second stage for the stride-2 kernel -- 2.10 ms against 1.81 ms on cfg 2, the L2 latency
-// outweighs the sparser bitmap: profiles/r02a_ab_*.jsonl, r02b_cfg3.jsonl, r02f_cfg2.jsonl.)
+// (Tried and dropped: a lane-local second stage without compaction, a paired one, and the
+// anchor-map second stage for the stride-2 kernel -- slower on cfg 2, the L2 latency outweighs the
+// sparser bitmap.)
 // Tile distribution DYN:
-//   0  static: warp w of a CTA takes the tiles w, w + W, w + 2W, ... of the CTA's chunk.  ncu (r02a):
-//      27.8 of 32 warps active on average, the least busy SM sub-partition active 74 % of the kernel --
-//      the scheduler favours some warps, nothing hands their neighbours' work over, and the kernel
-//      ends with its slowest warp.
+//   0  static: warp w of a CTA takes the tiles w, w + W, w + 2W, ... of the CTA's chunk.  The
+//      scheduler favours some warps, nothing hands their neighbours' work over, and the kernel ends
+//      with its slowest warp.
 //   1  (default) the warps of a CTA draw tiles of the CTA's chunk from a shared-memory counter, four
-//      per atomic: -9 % on cfg 2, -7 % cfg 3, -15 % cfg 5 against the static split.
+//      per atomic: faster than the static split on cfg 2, cfg 3 and cfg 5.
 //   2  tiles numbered over the whole region, super-tiles of 256 per CTA from a global counter
 //      (prefetched half-way through the current one), batches of four per warp from a 64-bit
 //      shared-memory word.  A CTA that starts late or shares its SM with another kernel simply ends
 //      up with fewer super-tiles -- meant for the pipelined multi-GPU steps -- but the heavier draw
-//      costs what the better balance wins: 1.95 ms against 1.80 ms (1) and 1.97 ms (0) on cfg 2
-//      (profiles/r02k_*.jsonl, r02l_*.jsonl).  Kept selectable (ACG_EXP_GLOBAL_TILES).
+//      costs what the better balance wins: on cfg 2 it is slower than (1) and no faster than (0).
+//      Kept selectable (ACG_EXP_GLOBAL_TILES).
 template <int MODE, bool MASKED, bool DENSE, int STRIDE, int GEOM, int DYN = 0>
 __global__ void __launch_bounds__(PfGeom<GEOM>::kThreads, PfGeom<GEOM>::kMinCtas)  // wide: two CTAs per SM (64 registers)
 prefilter_kernel(DfaDev d, PrefilterLaunch p) {
@@ -306,20 +305,24 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   }
 
   // The chunk of the span this CTA's tile numbers refer to.  Static split: a contiguous 1/gridDim of
-  // the region, in units of 16-byte blocks.  DYN: the whole region -- tiles are handed out globally.
+  // the region, in units of 16-byte blocks (the brute-force path always takes it).  DYN 2: the whole
+  // region -- tiles are handed out globally -- known at compile time, so that its bounds stay launch
+  // parameters instead of registers.
   const uint64_t n_blocks16 = (p.region_hi - p.region_lo) >> 4;
   const uint64_t per_cta = (n_blocks16 + gridDim.x - 1) / gridDim.x;
   const uint64_t b0 = (uint64_t)blockIdx.x * per_cta;
   const uint64_t b1 = min(b0 + per_cta, n_blocks16);
-  const bool whole = DYN == 2 && !p.brute;
-  const uint64_t chunk_lo = whole ? p.region_lo : p.region_lo + (b0 << 4);
-  const uint64_t chunk_hi = whole ? p.region_hi : (b0 < b1 ? p.region_lo + (b1 << 4) : p.region_lo + (b0 << 4));
+  const uint64_t split_lo = p.region_lo + (b0 << 4);
+  const uint64_t split_hi = b0 < b1 ? p.region_lo + (b1 << 4) : split_lo;
 
   if (p.brute) {
-    for (uint64_t s = chunk_lo + tid; s < chunk_hi; s += kPfThreads) verify_at<MODE>(d, p, s_cls, s, em);
-    if (tid == 0 && chunk_hi > chunk_lo) atomicAdd(p.counter + 1, (unsigned long long)(chunk_hi - chunk_lo));
+    for (uint64_t s = split_lo + tid; s < split_hi; s += kPfThreads) verify_at<MODE>(d, p, s_cls, s, em);
+    if (tid == 0 && split_hi > split_lo) atomicAdd(p.counter + 1, (unsigned long long)(split_hi - split_lo));
     return;
   }
+  constexpr bool whole = DYN == 2;
+  const uint64_t chunk_lo = whole ? p.region_lo : split_lo;
+  const uint64_t chunk_hi = whole ? p.region_hi : split_hi;
 
   const uint32_t kmask = p.kmask, fold = p.fold, mult = p.mult;
   const uint32_t fold1 = p.fold & 0x00FFFFFFu;  // stride 2: the first stage fingerprints 3 bytes
@@ -475,7 +478,7 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
     if (t >= n_tiles) break;  // tile numbers only grow: nothing is in flight for this warp any more
     const uint64_t wbase = chunk_lo + (uint64_t)t * kPfTile;
     uint32_t win = 0;
-    if (use_windows) {  // (a chunk below 2 GiB -- every CTA chunk of a span under 296 GiB -- has one window)
+    if (use_windows) {  // (a chunk below 2 GiB -- every CTA chunk of a span under 264 GiB on 132 SMs -- has one window)
       win = (uint32_t)(((uint64_t)t * kPfTile) >> kWinShift);
       if (win != q2win) {  // warp-uniform
         if (q2len) drain2();

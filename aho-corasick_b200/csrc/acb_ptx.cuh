@@ -1,4 +1,4 @@
-// acb_ptx.cuh -- the inline-PTX primitives of the kernels (sm_100a), in one place:
+// acb_ptx.cuh -- the inline-PTX primitives of the kernels (sm_90a), in one place:
 // mbarrier + bulk async copy (TMA) for the haystack ring, shared-memory reads by 32-bit shared
 // address, the streaming global load of the walk kernel, and the kernel launch macro.
 //

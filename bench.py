@@ -1,16 +1,18 @@
 #!/usr/bin/env python3
 """bench.py -- BASELINE metric: GiB/s of haystack scanned (config 2: 5000 patterns, 4 GiB, DFA,
-MatchKind::Standard overlapping) on N B200s, with roofline / cpu_baseline / e2e objects.
+MatchKind::Standard overlapping) on N H100s, with roofline / cpu_baseline / e2e objects.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--hay-gib G] [--workload cfg2|cfg3|cfg4|cfg5]
-                    [--impl reference]
+                    [--impl reference] [--dump-outputs DIR]
 
 Our arm: every search goes through the C ABI of libacb200.so (ctypes).  N > 1: one process per GPU,
 acg_comm_init + acg_find_overlapping_sharded (haystack slices, records stored into rank 0's buffer
 over NVLink peer memory; NCCL for the counts / barrier) -- torch.distributed is only the launcher's
 rendezvous, barrier and max-over-ranks reduction of the timings.
 Reference arm (--impl reference): the reference's CPU loop (src/automaton.rs:1491-1534 over
-src/dfa.rs:218-226) as restated in oracle/ (kind "port": no rustc in this image), on the host cores.
+src/dfa.rs:218-226) as restated in oracle/ (kind "port": the Rust crate itself is not built), on the
+host cores.
+--dump-outputs DIR: after the timed steps, the ordered match list of the last step as DIR/*.npy (dump_outputs).
 """
 import argparse
 import importlib.util
@@ -23,6 +25,7 @@ import time
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent
+sys.dont_write_bytecode = True  # the tree may be read-only: nothing is cached in it
 GIB = float(1 << 30)
 DESC = {"cfg2": "5000 random 4-16B printable-ASCII patterns, DFA, MatchKind::Standard, find_overlapping_iter",
         "cfg3": "5000 patterns, ascii_case_insensitive, DFA, MatchKind::LeftmostFirst, find_iter",
@@ -43,15 +46,24 @@ def peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         return json.loads(p.read_text())["hbm_gbs"], "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet (HBM3, not reached)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks during the timed region, and the card's name and power limit (a number means
+    little without them)."""
 
     def __init__(self, index=0):
         self.samples, self.reasons, self._stop, self.index = [], set(), threading.Event(), index
         self.max_mhz = None
+        self.card = {}
+        try:
+            out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits",
+                                  "-i", str(index)], capture_output=True, text=True, timeout=10).stdout
+            name, limit = [x.strip() for x in out.strip().split(",")]
+            self.card = {"gpu": name, "power_limit_w": float(limit)}
+        except Exception:
+            pass
 
     def _run(self):
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -83,7 +95,7 @@ class ClockSampler:
     def summary(self):
         s = sorted(self.samples)
         return {"sm_mhz": s[len(s) // 2] if s else None, "sm_max_mhz": self.max_mhz,
-                "reasons": sorted(self.reasons)}
+                "reasons": sorted(self.reasons), **self.card}
 
 
 def usable_cores():
@@ -191,8 +203,8 @@ def reference_arm(args):
             "data": "synthetic", "same_config": False, "kind": "port",
             "config": {"workload": f"{wl}: {DESC[wl]}; bounded sample of the synthetic haystack",
                        "sample_bytes": sample,
-                       "note": "C restatement of src/automaton.rs:1491-1534 over src/dfa.rs:218-226 (no rustc in "
-                               "the image); the reference itself is single-threaded -- see one_thread_value"},
+                       "note": "C restatement of src/automaton.rs:1491-1534 over src/dfa.rs:218-226 (the Rust "
+                               "crate is not built); the reference itself is single-threaded -- see one_thread_value"},
             "one_thread_value": one_thread, "matches_in_sample": n1,
             "cpu_baseline": {"value": val, "unit": "GiB/s", "cores": cores, "kind": "port",
                              "one_thread_value": one_thread,
@@ -247,8 +259,27 @@ class Rig:
         return int(t.item())
 
 
-def run_workload(rig, args, wl, steps, warmup, want_e2e=True, check=True):
-    """Device-resident and end-to-end throughput of one workload on rig.world GPUs."""
+def dump_outputs(out_dir, rec):
+    """The ordered match list a caller of the timed path receives, as float64 pid / start / end arrays
+    (DIR/<name>.npy) plus count.npy.  Under 64 MB in all: beyond 1.9 million matches a fixed seeded
+    sample of the list is written, with the sampled positions in index.npy."""
+    import numpy as np
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    n = len(rec)
+    limit = 1_900_000  # four float64 arrays: 60.8 MB, headers included under 64 * 10^6 bytes
+    np.save(out / "count.npy", np.array([n], dtype=np.float64))
+    if n > limit:
+        idx = np.sort(np.random.default_rng(0).choice(n, limit, replace=False))
+        rec = rec[idx]
+        np.save(out / "index.npy", idx.astype(np.float64))
+    for k in ("pid", "start", "end"):
+        np.save(out / f"{k}.npy", rec[k].astype(np.float64))
+
+
+def run_workload(rig, args, wl, steps, warmup, want_e2e=True, check=True, dump=None):
+    """Device-resident and end-to-end throughput of one workload on rig.world GPUs.  dump: directory for
+    the outputs of the last timed step (dump_outputs)."""
     import numpy as np
     import aho_corasick_b200 as ab
     from aho_corasick_b200 import sharded as S
@@ -304,6 +335,7 @@ def run_workload(rig, args, wl, steps, warmup, want_e2e=True, check=True):
                 else:
                     r, ms = ac.find_iter_dev_np(d_hay.data_ptr(), n_local, span)
                     n = len(r)
+                    state["last"] = r
                 return n, ms, 0.0, None
             except OverflowError as e:
                 state["cap"] = int(e.args[0]) * 9 // 8 + 1024
@@ -370,6 +402,16 @@ def run_workload(rig, args, wl, steps, warmup, want_e2e=True, check=True):
                 gather_ms.append(gms)
         rig.barrier()
         wall = time.perf_counter() - t0
+    if dump and rank == 0:
+        # what the last timed step left for its caller: rank 0's gathered list (N > 1), the records in the
+        # device buffer (overlapping) or the returned list (find_iter)
+        if world > 1:
+            rec = rig.comm.fetch()
+        elif overlapping:
+            rec = state["out"][: cnt * ab.MATCH_DTYPE.itemsize].cpu().numpy().view(ab.MATCH_DTYPE)
+        else:
+            rec = state["last"]
+        dump_outputs(dump, rec)
     stats = ac.last_stats()
     if mode == "stream":
         # one pair of CUDA events around the K overlapped steps, taken inside the library after the
@@ -420,7 +462,7 @@ def run_workload(rig, args, wl, steps, warmup, want_e2e=True, check=True):
         for _ in range(2):
             n_e2e = e2e_step(h_np)
         rig.barrier()
-        e2e_steps = max(2, min(steps, 4))
+        e2e_steps = steps
         t0 = time.perf_counter()
         for _ in range(e2e_steps):
             n_e2e = e2e_step(h_np)
@@ -507,7 +549,11 @@ def main():
     ap.add_argument("--host-fill", action="store_true", help="cfg5: build the dense table on the host")
     ap.add_argument("--experiment", type=int, default=0,
                     help="ACG_EXP_* flags (include/acb200_debug.h); 0 = default kernel")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's match list as DIR/{pid,start,end,count}.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return reference_arm(args)
 
@@ -515,7 +561,7 @@ def main():
     rig = Rig(args)
     world, rank = rig.world, rig.rank
     wl = args.workload
-    main_res = run_workload(rig, args, wl, args.steps, args.warmup, want_e2e=True)
+    main_res = run_workload(rig, args, wl, args.steps, args.warmup, want_e2e=True, dump=args.dump_outputs)
     extras = {}
     if not args.no_extras and not args.experiment and wl == "cfg2":
         # the other BASELINE configs, device-resident, so that the driver-run line carries them:
@@ -523,7 +569,7 @@ def main():
         for x in (["cfg3", "cfg4", "cfg5"] if world == 1 else ["cfg5"]):
             saved = args.no_cpu_baseline
             args.no_cpu_baseline = True
-            r = run_workload(rig, args, x, max(3, min(args.steps, 5)), 3, want_e2e=(x == "cfg5" and world > 1), check=True)
+            r = run_workload(rig, args, x, args.steps, 3, want_e2e=(x == "cfg5" and world > 1), check=True)
             args.no_cpu_baseline = saved
             extras[x] = r
     if rank != 0:
@@ -535,17 +581,8 @@ def main():
     kname = {1: "walk_overlapping_kernel", 2: "prefilter_kernel", 3: "seq_find_kernel"}
 
     def roofline(r):
-        k = kname[r["engine"]]
-        traffic, src = None, None
-        tf = ROOT / "profiles" / "dram_traffic.json"
-        if tf.exists():
-            rec = json.loads(tf.read_text()).get(f"{r['workload']}:{k}")
-            if rec:  # `ncu --set full` of this kernel (dram__bytes_read.sum + dram__bytes_write.sum per
-                     # haystack byte of one launch), scaled to this launch's bytes; not measured by this run
-                traffic, src = rec["dram_bytes_per_haystack_byte"] * r["n_bytes"], rec["source"]
         return {"bound": "hbm", "achieved": r["achieved"], "peak": peak, "unit": "GB/s", "frac": r["achieved"] / peak,
-                "traffic": traffic, "traffic_source": src, "peak_source": which, "kernel": k,
-                "algorithmic_bytes_per_launch": r["n_bytes"]}
+                "peak_source": which, "kernel": kname[r["engine"]], "algorithmic_bytes_per_launch": r["n_bytes"]}
     r = main_res
     line = {
         "metric": "haystack_scan_throughput", "value": r["value"], "unit": "GiB/s", "n_gpus": world,
@@ -555,7 +592,7 @@ def main():
         "config": {"workload": f"{wl}: {DESC[wl]}; {r['per_gpu'] / GIB:g} GiB synthetic haystack per GPU, "
                                "~1 planted pattern per 4 KiB",
                    "haystack_bytes_per_gpu": r["per_gpu"], "global_haystack_bytes": r["total"],
-                   "l2": "input per launch is far larger than the 126 MB L2",
+                   "l2": "input per launch is far larger than the 50 MB L2",
                    "engine": kname[r["engine"]], "experiment": args.experiment, "device_fill": r["device_fill"],
                    "table_bytes": r["table_bytes"], "states": r["states"],
                    "sharding": (f"haystack slices, max_pattern_len-1 overlap, " + SHARDING[r["step_mode"]] +

@@ -1,5 +1,5 @@
 /*
- * acb200.h -- C ABI of the B200-native Aho-Corasick search path (libacb200.so).
+ * acb200.h -- C ABI of the GPU-native Aho-Corasick search path (libacb200.so).
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  The reference has no
  * FFI in-tree; the seam its hot path sits behind is the sealed trait

@@ -45,14 +45,13 @@ int acg_debug_set_pipeline_chunk(acg_dfa* dfa, uint64_t bytes);
 
 /* Kernel / plan variants that never change results, only which instantiation of the prefilter kernel
  * runs or how its first-stage keys are formed; kept switchable so that tools/ab_inproc.py can time
- * them against each other in one process.  (The r01 variants TALL = 1, PAIR = 2, WALK_HOT = 4 and
- * LOCAL2 = 16, and an anchor-map second stage for the stride-2 kernel, were measured in r02 --
- * profiles/r02a_ab_*.jsonl, r02b_*.jsonl, r02f_*.jsonl -- lost, and are gone.) */
+ * them against each other in one process.  (Earlier variants TALL = 1, PAIR = 2, WALK_HOT = 4 and
+ * LOCAL2 = 16, and an anchor-map second stage for the stride-2 kernel, lost such comparisons and
+ * are gone.) */
 #define ACG_EXP_KEY24 8u         /* stride-2 first stage keyed by the 3 fingerprint bytes only; default: 27 bits (3 bytes +
                                   * low 3 bits of the fourth).  Rebuilds the bitmap. */
 #define ACG_EXP_STATIC_TILES 32u /* warp w of a CTA takes tiles w, w + W, ...; default: the warps of a CTA draw their tiles
-                                  * from a shared-memory counter.  r02 A/B (profiles/r02b_*.jsonl): dynamic tiles + 27-bit
-                                  * keys -7 % on cfg 2, -22 % on cfg 3, -15 % on cfg 5. */
+                                  * from a shared-memory counter. */
 #define ACG_EXP_GLOBAL_TILES 16u  /* tiles numbered over the whole region, super-tiles per CTA from a global counter */
 #define ACG_EXP_NO_BYTESCAN 64u  /* automata with a start-bytes / rare-bytes set: use the fingerprint filter anyway */
 int acg_debug_set_experiment(acg_dfa* dfa, uint32_t flags);

@@ -1,5 +1,5 @@
 /*
- * ac_oracle.h -- CPU oracle for the B200 Aho-Corasick hot path.
+ * ac_oracle.h -- CPU oracle for the GPU Aho-Corasick hot path.
  *
  * TEST INFRASTRUCTURE ONLY.  This is a plain-C restatement of the reference
  * algorithm (BurntSushi/aho-corasick 1.1.3) for the DFA-scan / packed hot path.
@@ -11,11 +11,10 @@
  * Parity status: PINNED against the reference's own golden vectors
  * (src/tests.rs:96-642, src/packed/tests.rs:129-368 incl. the 3x261 "Z"
  * padding variations, README/doc examples) via tests/test_oracle_golden.py.
- * The reference itself cannot be compiled here (no rustc/cargo), so there is
- * no oracle/_ref.
+ * The reference itself (Rust) is not built, so there is no oracle/_ref.
  *
  * Every function cites the reference file:line it restates (paths relative to
- * /root/reference).
+ * the root of the reference crate).
  */
 #ifndef AC_ORACLE_H
 #define AC_ORACLE_H

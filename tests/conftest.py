@@ -13,7 +13,7 @@ if str(ROOT / "tests") not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100)")
     # The oracle is test infrastructure: build it on demand (gcc only, ~1 s).
     so = ROOT / "oracle" / "libac_oracle.so"
     src = ROOT / "oracle" / "ac_oracle.c"

@@ -4,7 +4,7 @@
 // their *logic* (tile/chunk partitioning, ownership of start offsets, queues, ordering keys, the
 // host glue around them) can be checked against the oracle without a GPU.  It models none of the
 // hardware's concurrency or memory model and says nothing about performance; the real `-m gpu`
-// suite on a B200 remains the parity gate.
+// suite on an H100 remains the parity gate.
 //
 // Execution model: one CTA at a time; every CUDA thread of the CTA is a fiber (ucontext) scheduled
 // round-robin and switched only at warp/CTA collectives and mbarrier waits.  "Device memory" is

@@ -9,7 +9,7 @@ replace/stream glue, packed wrapper) be exercised on a machine without a GPU:
     ACB_FAKE_DEVICE=1 python -m pytest tests/test_gpu_zz_packed.py tests/test_gpu_parity.py -k "..."
 
 Tests that use device-resident haystacks (torch.cuda, *_dev entry points) cannot run this way.
-A pass here says nothing about the kernels; the real `-m gpu` run on a B200 does.
+A pass here says nothing about the kernels; the real `-m gpu` run on an H100 does.
 """
 import ctypes as C
 

@@ -1,13 +1,13 @@
 #!/usr/bin/env python3
 """Transcribe the reference's golden search vectors into language-neutral JSON.
 
-Run in the build container (the reference tree is NOT present on the GPU box):
+Run against a checkout of the reference crate (the tests only read the JSON written here):
 
-    python tests/golden/extract_vectors.py /root/reference tests/golden
+    python tests/golden/extract_vectors.py <reference checkout> tests/golden
 
 Sources (data only, no code is copied):
-  * /root/reference/src/tests.rs:96-642        -> ac_vectors.json
-  * /root/reference/src/packed/tests.rs:129-368 -> packed_vectors.json
+  * src/tests.rs:96-642        -> ac_vectors.json
+  * src/packed/tests.rs:129-368 -> packed_vectors.json
 
 Every `t!(name, &[patterns], "haystack", &[(pid, start, end), ...])` record in
 a `const GROUP: &'static [SearchTest]` block becomes
@@ -120,7 +120,9 @@ def parse_file(path: Path):
 
 
 def main():
-    ref = Path(sys.argv[1] if len(sys.argv) > 1 else "/root/reference")
+    if len(sys.argv) < 2:
+        sys.exit("usage: extract_vectors.py <reference checkout> [out dir]")
+    ref = Path(sys.argv[1])
     out = Path(sys.argv[2] if len(sys.argv) > 2 else Path(__file__).parent)
     for src, dst in [("src/tests.rs", "ac_vectors.json"),
                      ("src/packed/tests.rs", "packed_vectors.json")]:

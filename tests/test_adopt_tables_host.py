@@ -40,8 +40,14 @@ def test_oracle_tables_are_adopted(idx):
     for k in ("trans", "byte_classes", "match_offsets", "match_pids", "pattern_lens"):
         assert np.array_equal(np.asarray(got[k]), np.asarray(t[k])[: len(got[k])]), k
     assert ac.patterns_len() == len(pats) and ac.match_kind() == kw.get("match_kind", 0)
-    with pytest.raises(ab.DeviceError):   # no device here: adopted, but searches need the GPU
-        ac.find_iter(b"xx")
+    hay = b"xx " + b" ".join(pats[:20])
+    if ab.device_count() == 0:
+        with pytest.raises(ab.DeviceError):   # no device: adopted, but searches need the GPU
+            ac.find_iter(hay)
+    else:   # with a device the adopted table searches like the oracle
+        want = o.find_iter_np(np.frombuffer(hay, dtype=np.uint8))
+        assert [m.as_tuple() for m in ac.find_iter(hay)] == \
+            [(int(w["pid"]), int(w["start"]), int(w["end"])) for w in want]
 
 
 def _valid():

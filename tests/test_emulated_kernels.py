@@ -5,7 +5,7 @@ This is a check of the kernels' *logic* -- chunk/tile partitioning, ownership of
 every alignment, the stride-1 / stride-2 / wide / dense variants, queues and overflow paths,
 ordering keys, chain resolution, the device-resident and sharded entry points, the pipelined host
 path -- on machines without a GPU.  It models neither the hardware's concurrency nor its memory
-model; the `-m gpu` suite on a B200 remains the parity gate."""
+model; the `-m gpu` suite on an H100 remains the parity gate."""
 import ctypes
 import sys
 from pathlib import Path

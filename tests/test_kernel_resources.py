@@ -18,7 +18,7 @@ def ptxas_info(source):
     if not Path(nvcc).exists():
         pytest.skip("nvcc not available")
     with tempfile.TemporaryDirectory() as tmp:
-        r = subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-Xptxas", "-v",
+        r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
                             "-c", str(CSRC / source), "-o", str(Path(tmp) / "o.o")], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     out = {}
