@@ -28,7 +28,8 @@
 namespace acb {
 namespace {
 
-// Kernel geometry.  NARROW (0): 1 024 threads, 1 KiB tile per warp step (2 x 16 positions per lane);
+// Kernel geometry.  NARROW (0): 1 024 threads, 1 KiB tile per warp step (2 x 16 positions per lane;
+// stride 2 takes two such tiles per step, see PfPass);
 // WIDE (1, stride 2 only): 512 threads, 2 KiB tile per warp step (4 x 16 positions per lane, 32
 // probes), 16 KiB bitmap, two CTAs per SM -- the per-step bookkeeping is spread over twice as many
 // positions, which pays when first-stage hits are rare (few patterns); with frequent hits the 32
@@ -83,6 +84,20 @@ constexpr uint32_t kWinShift = 31;
 #endif
 
 constexpr int kPfStages = 2;            // ring depth per warp (TMA bulk copies + mbarriers, acb_ptx.cuh)
+
+// The haystack bytes one warp step probes before it compacts their hits.  Stride 2 on the narrow
+// geometry takes 2 KiB per step -- both 1 KiB halves of the warp's ring, filled by one bulk copy --
+// so that each lane collects 32 hit bits, as the wide geometry does: the ballots, syncs and loop
+// set-up of the hit path, the tile draw and the copy issue are paid once per 2 KiB instead of once
+// per KiB.  The ring is then a single stage (the warp waits for its next 2 KiB, the other 31 warps
+// of the SM issue meanwhile).  Stride 1 has 32 hit bits per lane with 1 KiB already.
+template <int GEOM, int STRIDE> struct PfPass {
+  static constexpr bool kPair = STRIDE == 2 && GEOM == kGeomNarrow;
+  static constexpr int kStages = kPair ? 1 : kPfStages;               // ring stages in use
+  static constexpr int kGroups = PfGeom<GEOM>::kGroups * (kPair ? 2 : 1);  // 16-byte groups per lane and step
+  static constexpr int kTile = kGroups * 512;                           // haystack bytes per warp step
+  static_assert(kStages * (kTile + 16) <= kPfStages * PfGeom<GEOM>::kStageBytes, "a step's tiles fit the warp's ring");
+};
 
 struct Emitter {
   uint64_t* g_keys;
@@ -253,17 +268,19 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   constexpr bool ANCH = DENSE;  // second stage = anchor-map lookup, queue entries carry the trie state
   constexpr int kPfThreads = PfGeom<GEOM>::kThreads;
   constexpr int kPfWarps = PfGeom<GEOM>::kWarps;
-  constexpr int kPfTile = PfGeom<GEOM>::kTile;
-  constexpr int kPfStageBytes = PfGeom<GEOM>::kStageBytes;
-  constexpr int kGroups = PfGeom<GEOM>::kGroups;
+  constexpr int kRingBytes = kPfStages * PfGeom<GEOM>::kStageBytes;  // per warp
+  constexpr int kStages = PfPass<GEOM, STRIDE>::kStages;
+  constexpr int kPfTile = PfPass<GEOM, STRIDE>::kTile;
+  constexpr int kPfStageBytes = kPfTile + 16;  // + fingerprint look-ahead
+  constexpr int kGroups = PfPass<GEOM, STRIDE>::kGroups;
   constexpr int kPfSlots = PfCfg<DENSE>::kSlots;
   constexpr int kSlotsAlloc = kPfSlots;
   constexpr int kPfQ2 = PfCfg<ANCH>::kQ2;
   constexpr uint32_t kBloomShift = PfBloom<GEOM>::kShift;
   using Q2Entry = typename std::conditional<ANCH, uint2, uint32_t>::type;  // (offset[, trie state of its first k bytes])
   ACB_DYNAMIC_SMEM(smem_raw);
-  unsigned char* s_ring = smem_raw;                                    // [kPfWarps][kPfStages][kPfStageBytes]
-  uint64_t* s_bars = reinterpret_cast<uint64_t*>(s_ring + kPfWarps * kPfStages * kPfStageBytes);  // [kPfWarps][kPfStages]
+  unsigned char* s_ring = smem_raw;                                    // [kPfWarps][kRingBytes]
+  uint64_t* s_bars = reinterpret_cast<uint64_t*>(s_ring + kPfWarps * kRingBytes);  // [kPfWarps][kPfStages]
   uint32_t* s_tile_of = reinterpret_cast<uint32_t*>(s_bars + kPfWarps * kPfStages);  // DYN: tile number staged in [warp][stage]
   uint32_t* s_next_tile = s_tile_of + kPfWarps * kPfStages;                        // DYN: draw state (u64), prefetched super-tile (u32), pad
   Q2Entry* s_queue2 = reinterpret_cast<Q2Entry*>(s_next_tile + 4);  // [kPfWarps][kPfQ2]
@@ -336,7 +353,7 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   const uint64_t chunk_base = chunk_lo - (uint64_t)(STRIDE - 1);
   const uint32_t rel_bias = (uint32_t)(STRIDE - 1);
   const uint8_t* s_bytes = reinterpret_cast<const uint8_t*>(s_bitmap);
-  unsigned char* ring = s_ring + warp * (kPfStages * kPfStageBytes);
+  unsigned char* ring = s_ring + warp * kRingBytes;
   uint64_t* bars = s_bars + warp * kPfStages;
   uint16_t* slots = s_slots + warp * kSlotsAlloc;
   Q2Entry* q2 = s_queue2 + warp * kPfQ2;
@@ -460,18 +477,18 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   if (lane == 0) {
     if constexpr (DYN) {
       draw(0);
-      draw(1);
+      if (kStages > 1) draw(1);
     } else {
       if ((uint32_t)warp < n_tiles) issue((uint32_t)warp, 0);
-      if ((uint32_t)warp + kPfWarps < n_tiles) issue((uint32_t)warp + kPfWarps, 1);
+      if (kStages > 1 && (uint32_t)warp + kPfWarps < n_tiles) issue((uint32_t)warp + kPfWarps, 1);
     }
   }
   __syncwarp();
   constexpr int kBitsPerGroup = 16 / STRIDE;
   constexpr int kHitBits = kGroups * kBitsPerGroup;
   for (uint32_t it = 0;; ++it) {
-    const uint32_t stage = it & 1;
-    const uint32_t parity = (it >> 1) & 1;
+    const uint32_t stage = kStages == 1 ? 0u : it & 1;
+    const uint32_t parity = (kStages == 1 ? it : it >> 1) & 1;
     uint32_t t;
     if constexpr (DYN) t = *reinterpret_cast<volatile uint32_t*>(tile_of + stage);
     else t = (uint32_t)warp + it * (uint32_t)kPfWarps;
@@ -689,11 +706,12 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
         }
       }
     }
-    __syncwarp();  // every lane is done with this stage: refill it with the tile two steps ahead
+    __syncwarp();  // every lane is done with this stage: refill it with the tile kStages steps ahead
     if (lane == 0) {
       if constexpr (DYN) draw(stage);
-      else if (t + 2 * kPfWarps < n_tiles) issue(t + 2 * kPfWarps, stage);
+      else if (t + kStages * kPfWarps < n_tiles) issue(t + kStages * kPfWarps, stage);
     }
+    if constexpr (DYN && kStages == 1) __syncwarp();  // the tile number just drawn is the next step's
   }
   if constexpr (DYN == 2) { if (lane == 0) publish(); }  // a prefetched super-tile index somebody may be waiting for
   if (q2len) drain2();
@@ -915,11 +933,11 @@ cudaError_t launch_prefilter(const DfaDev& dfa, const PrefilterLaunch& p, int sm
   const size_t bitmap_bytes = p.brute ? 0 : (size_t(1) << (p.log_bits - 3));
   static const int kThreadsOf[2] = {PfGeom<0>::kThreads, PfGeom<1>::kThreads};
   static const int kStageOf[2] = {PfGeom<0>::kStageBytes, PfGeom<1>::kStageBytes};
-  static const int kTileOf[2] = {PfGeom<0>::kTile, PfGeom<1>::kTile};
   const int threads = kThreadsOf[geom];
   const int warps = threads / 32;
   const int stage_bytes = kStageOf[geom];
-  const int tile = kTileOf[geom];
+  const int tile = geom == kGeomWide ? PfPass<kGeomWide, 2>::kTile
+                   : p.stride == 2 ? PfPass<kGeomNarrow, 2>::kTile : PfPass<kGeomNarrow, 1>::kTile;  // bytes per warp step
   const int q2_bytes = dense ? PfCfg<true>::kQ2 * 8 : PfCfg<false>::kQ2 * 4;
   const int slot_bytes = PfCfg<false>::kSlots * 2;
   const size_t smem = size_t(warps) * (kPfStages * stage_bytes + kPfStages * 12 + q2_bytes + slot_bytes) + 16 + bitmap_bytes;
