@@ -37,6 +37,10 @@ namespace {
     }                                                                                  \
   } while (0)
 
+// counters of a search: [0] tuples (bucketed emission: the overflow list), [1] candidates, [2] super-tiles,
+// [kBucketCountersAt + b] the tuples of bucket b
+constexpr size_t kCounterBytes = 8 * (acb::kBucketCountersAt + acb::kMaxBuckets);
+
 struct Workspace {
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
@@ -143,8 +147,8 @@ int init_workspace(Workspace& w) {
   CK(cudaEventCreate(&w.ev1));
   CK(cudaEventCreate(&w.ev2));
   CK(cudaEventCreate(&w.ev3));
-  CK(cudaMalloc(&w.d_counter, 64));
-  CK(cudaMallocHost(&w.h_counter, 64));
+  CK(cudaMalloc(&w.d_counter, kCounterBytes));
+  CK(cudaMallocHost(&w.h_counter, kCounterBytes));
   return ACG_OK;
 }
 
@@ -857,10 +861,54 @@ int run_walk_overlapping(const acg_dfa* a, const uint8_t* d_hay, uint64_t readab
   return ACG_E_NOMEM;
 }
 
+// Bucketed emission of the prefilter engine (PrefilterLaunch::bucket_shift): the span's key offsets
+// [0, n_bytes] are cut into `n` ranges of 2^shift bytes, fixed before the first launch, and each
+// bucket is given 2^log slots of tuple buffer 0, so that K4 is one shared-memory sort per bucket
+// (order_buckets_kernel) instead of a radix sort of the whole list.
+// The shift: 2^25 bytes (32 MiB) -- about 8 K tuples at the BASELINE density of one match per 4 KiB,
+// half of what one CTA sorts (kOrderCap = 16 K) -- unless the 32-bit sort key needs smaller buckets
+// (2^shift << tie_bits <= 2^32) or more than kMaxBuckets of them would be needed (then larger ones).
+// When the tie-break needs more than 10 bits (patterns of 1 KiB and more, or many duplicates) the
+// buckets would be under 4 MiB and their slots would outnumber the list's default capacity (one
+// tuple per 256 bytes): the single list and the radix sort then stay.  So do the walk engine and
+// the global super-tile distribution.  A bucket that fills up sends its further tuples to an
+// overflow list behind the buckets, and K4 falls back to the radix sort.
+struct BucketPlan {
+  uint32_t shift = 0;  // 0: a single list
+  uint32_t n = 0, log = 0, tie_bits = 0;  // buckets, log2 of the slots per bucket, bits of the tie-break
+  uint64_t slots() const { return uint64_t(n) << log; }
+};
+
+BucketPlan plan_buckets(const acg_dfa* a, uint64_t n_bytes) {
+  BucketPlan b;
+  if (a->experiment & ACG_EXP_GLOBAL_TILES) return b;
+  const uint32_t tie_bits = uint32_t(bits_for(a->h.max_pattern_len)) + a->pf.dup_shift;
+  if (tie_bits >= 32) return b;
+  const uint32_t max_shift = 32 - tie_bits;
+  uint32_t shift = std::min<uint32_t>(25, max_shift);
+  uint32_t min_shift = 22;
+  uint32_t log = acb::kOrderLog;
+#ifdef ACB_EMULATE
+  // dry run: smaller buckets / capacities, so that kilobyte inputs cross many buckets and overflow them
+  if (const char* e = getenv("ACB_EMU_BUCKETSHIFT")) { shift = std::min<uint32_t>(uint32_t(atoi(e)), max_shift); min_shift = 1; }
+  if (const char* e = getenv("ACB_EMU_BUCKETLOG")) log = std::min<uint32_t>(uint32_t(std::max(atoi(e), 0)), acb::kOrderLog);
+#endif
+  if (shift < min_shift) return b;
+  while ((n_bytes >> shift) + 1 > acb::kMaxBuckets) {
+    if (shift >= max_shift) return b;
+    ++shift;
+  }
+  b.shift = shift;
+  b.n = uint32_t((n_bytes >> shift) + 1);
+  b.log = log;
+  b.tie_bits = tie_bits;
+  return b;
+}
+
 // Enqueue one K3/K3b launch covering the start offsets [scan_lo, scan_hi) of the span.
 int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable,
                             uint64_t span_start, uint64_t span_end, uint64_t scan_lo,
-                            uint64_t scan_hi, int mode, int dev_sms) {
+                            uint64_t scan_hi, int mode, int dev_sms, const BucketPlan& bp) {
   Workspace& w = cur_ws();
   const PrefilterPlan& pf = a->pf;
   // 16-byte aligned filter region whose 4-byte look-ahead stays inside the readable bytes
@@ -902,6 +950,9 @@ int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t rea
   p.pids = w.d_pids[0];
   p.counter = w.d_counter;
   p.cap = w.cap;
+  p.bucket_shift = bp.shift;
+  p.bucket_log = bp.log;
+  p.bucket_slots = bp.slots();
   p.bs_n = 0;
   for (int i = 0; i < 3; ++i) { p.bs_needle[i] = 0; p.bs_back[i] = 0; }
   if (pf.bs_n && !a->bytescan_inert && !(a->experiment & ACG_EXP_NO_BYTESCAN)) {
@@ -917,27 +968,56 @@ int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t rea
   return ACG_OK;
 }
 
-// K4: order the appended tuples; `want` tuples sit in buffer 0.
-int order_tuples(const acg_dfa* a, uint64_t want, uint64_t n_bytes, TupleResult* res) {
+// K4: order the appended tuples; `want` tuples sit in buffer 0 -- as one list, or (bucketed) in the
+// buckets of `bp` and, `overflow` of them, in the overflow list behind the buckets.  Leaves them ordered
+// in buffer res->sorted_buf.  Everything between ev2 and ev3 is the order time.
+int order_tuples(const acg_dfa* a, uint64_t want, uint64_t n_bytes, TupleResult* res, const BucketPlan& bp,
+                 uint64_t overflow) {
   Workspace& w = cur_ws();
   res->n = want;
   cur_ws().stats.raw_matches = want;
-  if (want > 1) {
-    size_t tb = w.temp_bytes;
-    const int end_bit = std::min(64, acb::kTieBits + bits_for(n_bytes + 1));
-    float ms = 0;
-    CK(cudaEventRecord(w.ev2, w.stream));
+  res->sorted_buf = 0;
+  if (want <= 1 && (bp.shift == 0 || want == 0)) return ACG_OK;  // (one bucketed tuple still has to move to slot 0)
+  size_t tb = w.temp_bytes;
+  const int end_bit = std::min(64, acb::kTieBits + bits_for(n_bytes + 1));
+  float ms = 0;
+  CK(cudaEventRecord(w.ev2, w.stream));
+  if (bp.shift == 0) {
     CK(acb::sort_pairs(w.d_temp, tb, w.d_keys[0], w.d_keys[1], w.d_pids[0], w.d_pids[1], want, end_bit,
                        w.stream));
-    CK(cudaEventRecord(w.ev3, w.stream));
-    CK(cudaStreamSynchronize(w.stream));
-    cudaEventElapsedTime(&ms, w.ev2, w.ev3);
-    cur_ws().stats.order_ms = ms;
     cur_ws().stats.launches += 8;  // radix passes (library code, upper bound)
     res->sorted_buf = 1;
   } else {
-    res->sorted_buf = 0;
+    acb::OrderLaunch o;
+    o.keys_in = w.d_keys[0];
+    o.pids_in = w.d_pids[0];
+    o.keys_out = w.d_keys[1];
+    o.pids_out = w.d_pids[1];
+    o.bucket_count = w.d_counter + acb::kBucketCountersAt;
+    o.overflow_count = w.d_counter;
+    o.n_buckets = bp.n;
+    o.bucket_shift = bp.shift;
+    o.bucket_cap = 1u << bp.log;
+    o.tie_bits = bp.tie_bits;
+    o.bucket_slots = bp.slots();
+    if (overflow == 0) {
+      // every bucket within what one CTA sorts: the buckets' order is the keys' order already
+      CK(acb::launch_order_buckets(o, w.stream));
+      cur_ws().stats.launches += 1;
+      res->sorted_buf = 1;
+    } else {
+      // a bucket overflowed: concatenate buckets and overflow list, radix sort of the whole list
+      CK(acb::launch_compact_buckets(o, w.stream));
+      CK(acb::sort_pairs(w.d_temp, tb, w.d_keys[1], w.d_keys[0], w.d_pids[1], w.d_pids[0], want, end_bit,
+                         w.stream));
+      cur_ws().stats.launches += 9;
+      res->sorted_buf = 0;
+    }
   }
+  CK(cudaEventRecord(w.ev3, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+  cur_ws().stats.order_ms = ms;
   return ACG_OK;
 }
 
@@ -1056,15 +1136,19 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
   // one tuple per 256 haystack bytes to start with (the BASELINE workloads have one per 4 KiB);
   // denser outputs are detected through the counter and the scan is repeated with room
   uint64_t cap = std::max<uint64_t>(w.cap, std::max<uint64_t>(1 << 20, (scan_hi - scan_lo) / 256));
+  // bucketed emission: the buckets' slots, then at least 64 K slots of overflow list
+  const BucketPlan bp = plan_buckets(a, n_bytes);
+  cap = std::max<uint64_t>(cap, bp.slots() + (bp.shift ? (1u << 16) : 0));
+  const size_t counter_bytes = bp.shift ? 8 * (acb::kBucketCountersAt + size_t(bp.n)) : 16;
   bool copied = h_hay == nullptr;
   for (int attempt = 0; attempt < 8; ++attempt) {
     int rc = ensure_tuple_cap(w, cap);
     if (rc) return rc;
-    CK(cudaMemsetAsync(w.d_counter, 0, 16, w.stream));
+    CK(cudaMemsetAsync(w.d_counter, 0, counter_bytes, w.stream));
     CK(cudaEventRecord(w.ev0, w.stream));
     if (copied) {
       if ((rc = enqueue_prefilter_range(a, d_hay, readable, span_start, span_end, scan_lo, scan_hi, mode,
-                                        dev_sms)))
+                                        dev_sms, bp)))
         return rc;
     } else {
       // chunked H2D on the copy stream; a chunk's start offsets are scanned once the bytes a
@@ -1098,7 +1182,7 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
         const uint64_t upto = c1 == span_end ? span_end : (c1 > scanned + tail ? c1 - tail : scanned);
         if (upto > scanned || c1 == span_end) {
           if ((rc = enqueue_prefilter_range(a, d_hay, c1 == span_end ? readable : c1, span_start, span_end,
-                                            scanned, upto, mode, dev_sms)))
+                                            scanned, upto, mode, dev_sms, bp)))
             return rc;
           scanned = upto;
         }
@@ -1106,9 +1190,17 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
       copied = true;
     }
     CK(cudaEventRecord(w.ev1, w.stream));
-    CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 16, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaMemcpyAsync(w.h_counter, w.d_counter, counter_bytes, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaStreamSynchronize(w.stream));
-    const uint64_t want = w.h_counter[0];
+    // bucketed: counter[0] is the length of the overflow list, the buckets' counters include the tuples
+    // that went there
+    uint64_t want = w.h_counter[0], overflow = 0, room = w.cap;
+    if (bp.shift) {
+      overflow = want;
+      want = 0;
+      for (uint32_t i = 0; i < bp.n; ++i) want += w.h_counter[acb::kBucketCountersAt + i];
+      room = w.cap - bp.slots();
+    }
     cur_ws().stats.candidates = w.h_counter[1];
     // the reference retires a prefilter that keeps reporting candidates (PrefilterState,
     // src/util/prefilter.rs): needles in more than one offset out of 64 => fingerprint filter next time
@@ -1118,8 +1210,12 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
     float ms = 0;
     cudaEventElapsedTime(&ms, w.ev0, w.ev1);
     cur_ws().stats.scan_ms = ms;  // with a host haystack this is the overlapped copy+scan time
-    if (want > w.cap) { cap = want + want / 8 + 1024; continue; }
-    return order_tuples(a, want, n_bytes, res);
+    if (bp.shift ? overflow > room : want > w.cap) {
+      const uint64_t need = bp.shift ? overflow : want;
+      cap = (w.cap - room) + need + need / 8 + 1024;
+      continue;
+    }
+    return order_tuples(a, want, n_bytes, res, bp, overflow);
   }
   return ACG_E_NOMEM;
 }

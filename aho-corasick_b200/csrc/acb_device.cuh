@@ -135,7 +135,13 @@ struct PrefilterLaunch {
   uint32_t bs_back[3];
   uint32_t key_shift;           // stride 2: first-stage hash = window * (mult3 << key_shift).  8: the fourth window
                                 // byte drops out (3-byte keys); 5: its low 3 bits stay in the key (experiment).
-                                // Last member, so that the layout of the measured kernels' parameters is unchanged.
+  // Bucketed emission (bucket_shift != 0, see Emitter in acb_prefilter.cu): a tuple whose key offset is o goes to
+  // bucket o >> bucket_shift, slots [b << bucket_log, (b + 1) << bucket_log) of keys / pids, counted in
+  // counter[kBucketCountersAt + b]; a tuple whose bucket is full is appended to the overflow list behind the
+  // buckets (keys[bucket_slots + i], i counted in counter[0]).  0: one list counted in counter[0].
+  uint32_t bucket_shift;
+  uint32_t bucket_log;
+  uint64_t bucket_slots;        // n_buckets << bucket_log
 };
 cudaError_t launch_prefilter(const DfaDev& dfa, const PrefilterLaunch& p, int sm_count, cudaStream_t s);
 cudaError_t launch_bytescan(const DfaDev& dfa, const PrefilterLaunch& p, int sm_count, cudaStream_t s);
@@ -179,6 +185,30 @@ cudaError_t launch_expand(const ExpandLaunch& e, cudaStream_t s);
 // number of leading tuples whose end_rel <= bound (keys sorted ascending)
 cudaError_t launch_lower_bound(const uint64_t* keys, uint64_t n, uint64_t bound_key,
                                unsigned long long* d_result, cudaStream_t s);
+
+// K4 on bucketed tuples (PrefilterLaunch::bucket_shift).  Bucket b holds the keys with offsets in
+// [b << bucket_shift, (b + 1) << bucket_shift); its count is bucket_count[b] (may exceed bucket_cap: the rest
+// went to the overflow list).
+constexpr int kBucketCountersAt = 8;   // index of bucket 0's counter in the workspace's counter array
+constexpr uint32_t kMaxBuckets = 1024;
+constexpr uint32_t kOrderLog = 14;
+constexpr uint32_t kOrderCap = 1u << kOrderLog;  // tuples one CTA of order_buckets_kernel sorts in shared memory
+struct OrderLaunch {
+  const uint64_t* keys_in;             // buffer 0: bucket b at [b * bucket_cap, ...), then the overflow list
+  const uint32_t* pids_in;
+  uint64_t* keys_out;                  // [sum of the counts], (offset << 24 | tie, pid) ascending
+  uint32_t* pids_out;
+  const unsigned long long* bucket_count;  // [n_buckets]
+  const unsigned long long* overflow_count;
+  uint32_t n_buckets, bucket_shift, bucket_cap;
+  uint32_t tie_bits;                   // the tie-break occupies the low tie_bits bits of the key
+  uint64_t bucket_slots;               // n_buckets * bucket_cap: start of the overflow list
+};
+// One CTA per bucket sorts it in shared memory and stores it at the bucket's prefix offset.  Needs every
+// count <= bucket_cap <= kOrderCap (an empty overflow list).
+cudaError_t launch_order_buckets(const OrderLaunch& o, cudaStream_t s);
+// Fallback: the buckets and the overflow list, concatenated into keys_out / pids_out (unordered).
+cudaError_t launch_compact_buckets(const OrderLaunch& o, cudaStream_t s);
 
 // key/pid pair sort (K4). temp storage is queried with d_temp == nullptr.
 cudaError_t sort_pairs(void* d_temp, size_t& temp_bytes, const uint64_t* keys_in, uint64_t* keys_out,

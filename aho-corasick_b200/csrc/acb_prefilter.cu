@@ -99,23 +99,48 @@ template <int GEOM, int STRIDE> struct PfPass {
   static_assert(kStages * (kTile + 16) <= kPfStages * PfGeom<GEOM>::kStageBytes, "a step's tiles fit the warp's ring");
 };
 
+template <bool BUCKETED = true>  // false: the single list only (kernels that never bucket)
 struct Emitter {
   uint64_t* g_keys;
   uint32_t* g_pids;
   unsigned long long* g_counter;
   uint64_t cap;
+  uint32_t bucket_shift, bucket_log;  // see PrefilterLaunch
+  uint64_t bucket_slots;
   // Matches are sparse (about one per 4 KiB in the BASELINE workloads) while candidates are
   // verified by whole warps, so lanes that found something aggregate their append into one
   // atomic per warp step (warp-ballot + warp-aggregated atomic).
+  // Bucketed: the append goes to the bucket of the key's offset, so that the order step only sorts
+  // inside buckets (order_buckets_kernel).  A warp verifies offsets that lie close together, so its
+  // lanes nearly always share the bucket and keep the single atomic; lanes of different buckets
+  // append one by one.  A full bucket sends the tuple to the overflow list (never dropped; the order
+  // step then falls back to the radix sort of everything).
   __device__ __forceinline__ void emit(uint64_t key, uint32_t pid) {
     const unsigned m = __activemask();
     const int leader = __ffs(m) - 1;
     const int lane = threadIdx.x & 31;
-    unsigned long long base = 0;
-    if (lane == leader) base = atomicAdd(g_counter, (unsigned long long)__popc(m));
-    base = __shfl_sync(m, base, leader);
-    const unsigned long long g = base + __popc(m & ((1u << lane) - 1));
-    if (g < cap) { g_keys[g] = key; g_pids[g] = pid; }
+    const bool bucketed = BUCKETED && bucket_shift != 0;
+    unsigned long long* cnt = g_counter;
+    uint64_t first = 0;  // the bucket's first slot
+    bool together = true;
+    if (bucketed) {
+      const uint32_t b = (uint32_t)(key >> (kTieBits + bucket_shift));
+      cnt += kBucketCountersAt + b;
+      first = (uint64_t)b << bucket_log;
+      together = __ballot_sync(m, b == (uint32_t)__shfl_sync(m, b, leader)) == m;
+    }
+    unsigned long long g;
+    if (together) {
+      unsigned long long base = 0;
+      if (lane == leader) base = atomicAdd(cnt, (unsigned long long)__popc(m));
+      base = __shfl_sync(m, base, leader);
+      g = base + __popc(m & ((1u << lane) - 1));
+    } else {
+      g = atomicAdd(cnt, 1ull);
+    }
+    uint64_t slot = first + g;
+    if (bucketed && g >> bucket_log) slot = bucket_slots + atomicAdd(g_counter, 1ull);
+    if (slot < cap) { g_keys[slot] = key; g_pids[slot] = pid; }
   }
 };
 
@@ -160,9 +185,9 @@ __device__ __forceinline__ uint32_t anchor_lookup_key(const DfaDev& d, uint32_t 
 // Verify one candidate start offset `s` (K3b): walk the shipped DFA while the state stays on the
 // trie path anchored at s (depth == bytes consumed), starting from state `sid` at depth `j`
 // (the start state, or the state the anchor map gave for the first j bytes).
-template <int MODE>
+template <int MODE, class EM>
 __device__ __forceinline__ void verify_from(const DfaDev& d, const PrefilterLaunch& p, const uint8_t* s_cls,
-                                            uint64_t s, uint32_t sid, uint32_t j, Emitter& em) {
+                                            uint64_t s, uint32_t sid, uint32_t j, EM& em) {
   const uint8_t* __restrict__ hay = p.hay;
   const uint32_t* __restrict__ trans = d.trans;
   uint64_t pos = s + j;
@@ -200,9 +225,9 @@ __device__ __forceinline__ void verify_from(const DfaDev& d, const PrefilterLaun
   if (MODE == 1 && best_len) em.emit(((s - p.span_start) << kTieBits) | best_len, best_pid);
 }
 
-template <int MODE>
+template <int MODE, class EM>
 __device__ __forceinline__ void verify_at(const DfaDev& d, const PrefilterLaunch& p, const uint8_t* s_cls,
-                                          uint64_t s, Emitter& em) {
+                                          uint64_t s, EM& em) {
   if (d.amap != nullptr) {
     const uint32_t sid = anchor_lookup(d, p, s);
     if (sid != 0) verify_from<MODE>(d, p, s_cls, s, sid, d.amap_k, em);
@@ -305,7 +330,8 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   ptx::fence_proxy_async();
   __syncthreads();
 
-  Emitter em{p.keys, p.pids, p.counter, p.cap};
+  // (the global super-tile distribution keeps the single list, see plan_buckets in acb_api.cu)
+  Emitter<DYN != 2> em{p.keys, p.pids, p.counter, p.cap, p.bucket_shift, p.bucket_log, p.bucket_slots};
   unsigned long long cand_total = 0;
 
   // head / tail positions outside the aligned filter region are unconditional candidates
@@ -739,7 +765,7 @@ __global__ void __launch_bounds__(kBsThreads, 2) bytescan_kernel(DfaDev d, Prefi
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid < 256) s_cls[tid] = d.classes[tid];
   __syncthreads();
-  Emitter em{p.keys, p.pids, p.counter, p.cap};
+  Emitter<> em{p.keys, p.pids, p.counter, p.cap, p.bucket_shift, p.bucket_log, p.bucket_slots};
   unsigned long long cand_total = 0;
   // head / tail positions outside the aligned region are unconditional candidates
   if (blockIdx.x == 0) {
@@ -922,6 +948,170 @@ struct MaxOp {
   __device__ __forceinline__ uint64_t operator()(uint64_t a, uint64_t b) const { return a > b ? a : b; }
 };
 
+// ---- K4 on bucketed tuples ------------------------------------------------------------------------
+// The prefilter kernels append every tuple to the bucket of its key's offset (Emitter), so the buckets
+// are already in key order among themselves and only their insides need sorting: one CTA per bucket
+// loads it into shared memory as 32-bit keys ((offset - bucket base) << tie_bits | tie: the bucket's
+// range is planned to fit), sorts (key, 16-bit index) pairs by LSD radix with 8-bit digits, and stores
+// the tuples in their unchanged 64-bit form at the bucket's prefix offset.  One pass: every warp ranks
+// its own consecutive items (the lanes with the same digit found with eight ballots, a per-warp count
+// per digit in shared memory), the (digit, warp) counts are scanned in that order, and every item is
+// scattered to its digit's offset for its warp plus its rank -- stable, so the passes compose.
+constexpr int kOrdThreads = 1024;
+constexpr int kOrdWarps = kOrdThreads / 32;
+constexpr int kOrdRounds = (int)kOrderCap / kOrdThreads;  // items per lane and pass at most
+constexpr int kOrdBatch = 8;                               // global loads in flight per thread
+
+__global__ void __launch_bounds__(kOrdThreads, 1) order_buckets_kernel(OrderLaunch o) {
+  ACB_DYNAMIC_SMEM(smem_raw);
+  const uint32_t cap = o.bucket_cap;
+  uint32_t* ka = reinterpret_cast<uint32_t*>(smem_raw);  // [cap] x 2: keys, ping-pong
+  uint32_t* kb = ka + cap;
+  uint16_t* ia = reinterpret_cast<uint16_t*>(kb + cap);  // [cap] x 2: index of the tuple in the bucket
+  uint16_t* ib = ia + cap;
+  uint16_t* s_cnt = ib + cap;                            // [256 digits][kOrdWarps], then their exclusive scan
+  uint32_t* s_sum = reinterpret_cast<uint32_t*>(s_cnt + 256 * kOrdWarps);  // [kOrdWarps]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t lt = (1u << lane) - 1;
+  const uint32_t b = blockIdx.x;
+  const uint32_t n = (uint32_t)o.bucket_count[b];
+  if (n == 0) return;
+
+  // output offset: the tuples of the buckets before this one
+  uint32_t part = 0;
+  for (uint32_t i = tid; i < b; i += kOrdThreads) part += (uint32_t)o.bucket_count[i];
+  part = __reduce_add_sync(0xffffffffu, part);
+  if (lane == 0) s_sum[warp] = part;
+  __syncthreads();
+  uint64_t out0 = 0;
+  for (int w = 0; w < kOrdWarps; ++w) out0 += s_sum[w];
+
+  const uint64_t in0 = (uint64_t)b * cap;
+  const uint64_t off0 = (uint64_t)b << o.bucket_shift;
+  const uint32_t tie_bits = o.tie_bits;
+  const uint64_t tie_mask = (1ull << tie_bits) - 1;
+  for (uint32_t j0 = 0; j0 < n; j0 += kOrdBatch * kOrdThreads) {
+    uint64_t k[kOrdBatch];
+#pragma unroll
+    for (int u = 0; u < kOrdBatch; ++u) {
+      const uint32_t j = j0 + u * kOrdThreads + tid;
+      k[u] = j < n ? o.keys_in[in0 + j] : 0;
+    }
+#pragma unroll
+    for (int u = 0; u < kOrdBatch; ++u) {
+      const uint32_t j = j0 + u * kOrdThreads + tid;
+      if (j < n) {
+        ka[j] = (uint32_t)((((k[u] >> kTieBits) - off0) << tie_bits) | (k[u] & tie_mask));
+        ia[j] = (uint16_t)j;
+      }
+    }
+  }
+
+  // warp w ranks the items [w_lo, w_hi), 32 per round
+  const uint32_t per_warp = (n + kOrdWarps - 1) / kOrdWarps;
+  const uint32_t w_lo = min(warp * per_warp, n), w_hi = min(w_lo + per_warp, n);
+  const uint32_t rounds = (per_warp + 31) / 32;
+  const uint32_t key_bits = o.bucket_shift + tie_bits;
+  for (uint32_t sh = 0; sh < key_bits; sh += 8) {
+    for (int i = tid; i < 256 * kOrdWarps / 2; i += kOrdThreads) reinterpret_cast<uint32_t*>(s_cnt)[i] = 0;
+    __syncthreads();  // counts cleared, keys in place
+    uint32_t rd[kOrdRounds];  // digit << 16 | rank among the warp's items of that digit
+#pragma unroll
+    for (int r = 0; r < kOrdRounds; ++r) {
+      rd[r] = 0;
+      if ((uint32_t)r < rounds) {  // warp-uniform
+        const uint32_t i = w_lo + r * 32 + lane;
+        const bool valid = i < w_hi;
+        const uint32_t digit = valid ? (ka[i] >> sh) & 0xFFu : 0u;
+        uint32_t peers = __ballot_sync(0xffffffffu, valid);
+#pragma unroll
+        for (int bit = 0; bit < 8; ++bit) {
+          const uint32_t bb = __ballot_sync(0xffffffffu, (digit >> bit) & 1u);
+          peers &= ((digit >> bit) & 1u) ? bb : ~bb;
+        }
+        uint16_t* c = s_cnt + digit * kOrdWarps + warp;
+        const uint32_t base = valid ? *c : 0u;
+        __syncwarp();
+        if (valid && (peers & lt) == 0) *c = (uint16_t)(base + __popc(peers));
+        __syncwarp();
+        rd[r] = (digit << 16) | (base + __popc(peers & lt));
+      }
+    }
+    __syncthreads();
+    {  // exclusive scan of the counts in (digit, warp) order, 8 per thread
+      constexpr int kPer = 256 * kOrdWarps / kOrdThreads;
+      uint16_t* c = s_cnt + tid * kPer;
+      uint32_t v[kPer], sum = 0;
+#pragma unroll
+      for (int u = 0; u < kPer; ++u) { v[u] = c[u]; sum += v[u]; }
+      uint32_t incl = sum;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t x = (uint32_t)__shfl_sync(0xffffffffu, incl, lane >= d ? lane - d : lane);
+        if (lane >= d) incl += x;
+      }
+      if (lane == 31) s_sum[warp] = incl;
+      __syncthreads();
+      uint32_t run = incl - sum;
+      for (int w = 0; w < warp; ++w) run += s_sum[w];
+#pragma unroll
+      for (int u = 0; u < kPer; ++u) { c[u] = (uint16_t)run; run += v[u]; }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < kOrdRounds; ++r) {
+      const uint32_t i = w_lo + r * 32 + lane;
+      if ((uint32_t)r < rounds && i < w_hi) {
+        const uint32_t dst = s_cnt[(rd[r] >> 16) * kOrdWarps + warp] + (rd[r] & 0xFFFFu);
+        kb[dst] = ka[i];
+        ib[dst] = ia[i];
+      }
+    }
+    __syncthreads();  // scattered; the counts may be cleared
+    uint32_t* tk = ka; ka = kb; kb = tk;
+    uint16_t* ti = ia; ia = ib; ib = ti;
+  }
+
+  for (uint32_t j0 = 0; j0 < n; j0 += kOrdBatch * kOrdThreads) {
+    uint32_t pid[kOrdBatch];
+#pragma unroll
+    for (int u = 0; u < kOrdBatch; ++u) {
+      const uint32_t j = j0 + u * kOrdThreads + tid;
+      pid[u] = j < n ? o.pids_in[in0 + ia[j]] : 0u;
+    }
+#pragma unroll
+    for (int u = 0; u < kOrdBatch; ++u) {
+      const uint32_t j = j0 + u * kOrdThreads + tid;
+      if (j < n) {
+        const uint32_t sk = ka[j];
+        o.keys_out[out0 + j] = ((off0 + (sk >> tie_bits)) << kTieBits) | (sk & tie_mask);
+        o.pids_out[out0 + j] = pid[u];
+      }
+    }
+  }
+}
+
+// Fallback of the order step (a bucket overflowed): CTA b < n_buckets copies bucket b, CTA n_buckets
+// the overflow list, each to its prefix offset; the radix sort of the whole list follows.
+constexpr int kCompactThreads = 256;
+__global__ void __launch_bounds__(kCompactThreads) compact_buckets_kernel(OrderLaunch o) {
+  __shared__ unsigned long long s_part[kCompactThreads];
+  const uint32_t b = blockIdx.x;
+  const int tid = threadIdx.x;
+  unsigned long long part = 0;
+  for (uint32_t i = tid; i < b && i < o.n_buckets; i += kCompactThreads) part += min(o.bucket_count[i], (unsigned long long)o.bucket_cap);
+  s_part[tid] = part;
+  __syncthreads();
+  uint64_t dst = 0;
+  for (int i = 0; i < kCompactThreads; ++i) dst += s_part[i];
+  const uint64_t n = b < o.n_buckets ? min(o.bucket_count[b], (unsigned long long)o.bucket_cap) : *o.overflow_count;
+  const uint64_t src = b < o.n_buckets ? (uint64_t)b * o.bucket_cap : o.bucket_slots;
+  for (uint64_t j = tid; j < n; j += kCompactThreads) {
+    o.keys_out[dst + j] = o.keys_in[src + j];
+    o.pids_out[dst + j] = o.pids_in[src + j];
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_prefilter(const DfaDev& dfa, const PrefilterLaunch& p, int sm_count, cudaStream_t s) {
@@ -1000,7 +1190,21 @@ cudaError_t launch_chain_select(const ChainLaunch& c, cudaStream_t s) {
   ACB_LAUNCH(chain_select_kernel, blocks, 256, 0, s, c);
   return cudaGetLastError();
 }
-cudaError_t scan_max_u64(void* d_temp, size_t& temp_bytes, uint64_t* data, uint64_t n, cudaStream_t s) {
+cudaError_t launch_order_buckets(const OrderLaunch& o, cudaStream_t s) {
+  if (o.n_buckets == 0 || o.n_buckets > kMaxBuckets || o.bucket_cap == 0 || o.bucket_cap > kOrderCap ||
+      o.bucket_shift + o.tie_bits > 32)
+    return cudaErrorInvalidValue;
+  const size_t smem = size_t(o.bucket_cap) * 12 + 256 * kOrdWarps * 2 + kOrdWarps * 4;
+  cudaError_t e = cudaFuncSetAttribute(order_buckets_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  ACB_LAUNCH(order_buckets_kernel, o.n_buckets, kOrdThreads, smem, s, o);
+  return cudaGetLastError();
+}
+cudaError_t launch_compact_buckets(const OrderLaunch& o, cudaStream_t s) {
+  ACB_LAUNCH(compact_buckets_kernel, o.n_buckets + 1, kCompactThreads, 0, s, o);
+  return cudaGetLastError();
+}
+cudaError_t scan_max_u64(void* d_temp,size_t& temp_bytes, uint64_t* data, uint64_t n, cudaStream_t s) {
   return cub::DeviceScan::InclusiveScan(d_temp, temp_bytes, data, data, MaxOp(), (int64_t)n, s);
 }
 cudaError_t select_flagged(void* d_temp, size_t& temp_bytes, const uint64_t* keys_in, const uint32_t* pids_in,
