@@ -115,6 +115,7 @@ class _Stats(C.Structure):
 
 
 MATCH_DTYPE = np.dtype([("pid", "<u4"), ("_pad", "<u4"), ("start", "<u8"), ("end", "<u8")])
+DOC_MATCH_DTYPE = np.dtype([("pid", "<u4"), ("doc", "<u4"), ("start", "<u8"), ("end", "<u8")])  # acg_doc_match
 
 _vp, _u64, _i = C.c_void_p, C.c_uint64, C.c_int
 
@@ -149,6 +150,9 @@ def _declare(lib):
                                                C.POINTER(C.c_float)]
     lib.acg_find_overlapping_devout.argtypes = [_vp, _vp, _u64, _u64, _u64, _u64, _u64, _vp, _u64,
                                                  C.POINTER(_u64), C.POINTER(C.c_float)]
+    lib.acg_find_iter_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _vp, _u64, C.POINTER(_u64)]
+    lib.acg_find_overlapping_batch.argtypes = lib.acg_find_iter_batch.argtypes
+    lib.acg_is_match_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _vp]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -219,6 +223,30 @@ def _hay_ptr(hay):
         hay = hay.encode()
     arr = np.frombuffer(bytes(hay) if not isinstance(hay, (bytes, bytearray, memoryview)) else hay, dtype=np.uint8)
     return arr, arr.ctypes.data if arr.size else 0, arr.size
+
+
+def _batch_input(docs):
+    """(keepalive, address, length, on_device, uint64 offsets) of a batch of documents: a list of
+    bytes / str, or a (values, offsets) pair -- values a contiguous uint8 ndarray or a CUDA torch.uint8
+    tensor, offsets the [n_docs + 1] CSR bounds (host, int64)."""
+    if isinstance(docs, tuple) and len(docs) == 2:
+        values, offsets = docs
+        offs = np.ascontiguousarray(offsets, dtype=np.int64)
+        if offs.ndim != 1 or offs.size == 0 or (offs < 0).any():
+            raise ValueError("document offsets must be a non-empty 1-D array of non-negative integers")
+        offs = offs.astype(np.uint64)
+        if getattr(values, "is_cuda", False):
+            if str(values.dtype) != "torch.uint8" or not values.is_contiguous():
+                raise TypeError("device haystack must be a contiguous torch.uint8 tensor")
+            return values, values.data_ptr(), values.numel(), 1, offs
+        keep, ptr, n = _hay_ptr(values)
+        return keep, ptr, n, 0, offs
+    pieces = [d.encode() if isinstance(d, str) else bytes(d) for d in docs]
+    offs = np.zeros(len(pieces) + 1, dtype=np.uint64)
+    if pieces:
+        np.cumsum(np.fromiter(map(len, pieces), dtype=np.uint64, count=len(pieces)), out=offs[1:])
+    keep, ptr, n = _hay_ptr(b"".join(pieces))
+    return keep, ptr, n, 0, offs
 
 
 def _span(span, n):
@@ -627,6 +655,58 @@ class AhoCorasick:
         if isinstance(hay, Input):
             return self.try_find(hay.clone().earliest(earliest)) is not None
         return self.try_find(hay, span, earliest=earliest) is not None
+
+    # ---- batched search: many documents in one device call (include/acb200.h, acg_*_batch) ----
+    # `docs`: a list of bytes / str, or (values, offsets) with values a uint8 ndarray or a CUDA
+    # torch.uint8 tensor and offsets the host int64 CSR bounds [n_docs + 1].  Per document the results are
+    # those of the single-haystack call on that document alone, offsets relative to it.
+    def _collect_batch(self, fn, docs, anchored):
+        keep, ptr, n, on_dev, offs = _batch_input(docs)
+        n_docs = offs.size - 1
+        cap = max(self._cap_hint, n // 256 + 64)
+        while True:
+            out = np.empty(cap, DOC_MATCH_DTYPE)
+            cnt = _u64()
+            rc = fn(self._h, ptr, on_dev, n, offs.ctypes.data, n_docs, int(anchored), out.ctypes.data, cap,
+                    C.byref(cnt))
+            if rc == E_OVERFLOW:
+                cap = int(cnt.value) + int(cnt.value) // 8 + 64
+                self._cap_hint = max(self._cap_hint, cap)
+                continue
+            if rc:
+                self._raise(rc)
+            return out[: cnt.value], n_docs
+
+    @staticmethod
+    def _per_doc(r, n_docs):
+        res = [[] for _ in range(n_docs)]
+        for d, p, s, e in zip(r["doc"].tolist(), r["pid"].tolist(), r["start"].tolist(), r["end"].tolist()):
+            res[d].append(Match(p, s, e))
+        return res
+
+    def find_iter_batch_np(self, docs, anchored=Anchored.No):
+        """find_iter of every document: structured array (doc, pid, start, end), ascending doc."""
+        return self._collect_batch(_lib.acg_find_iter_batch, docs, anchored)[0]
+
+    def find_overlapping_iter_batch_np(self, docs, anchored=Anchored.No):
+        return self._collect_batch(_lib.acg_find_overlapping_batch, docs, anchored)[0]
+
+    def find_iter_batch(self, docs, anchored=Anchored.No):
+        """find_iter of every document: one list of Match per document."""
+        return self._per_doc(*self._collect_batch(_lib.acg_find_iter_batch, docs, anchored))
+
+    def find_overlapping_iter_batch(self, docs, anchored=Anchored.No):
+        return self._per_doc(*self._collect_batch(_lib.acg_find_overlapping_batch, docs, anchored))
+
+    def is_match_batch(self, docs, anchored=Anchored.No):
+        """is_match of every document: bool array [n_docs]."""
+        keep, ptr, n, on_dev, offs = _batch_input(docs)
+        flags = np.zeros(max(offs.size - 1, 1), dtype=np.uint8)
+        rc = _lib.acg_is_match_batch(self._h, ptr, on_dev, n, offs.ctypes.data, offs.size - 1, int(anchored),
+                                     flags.ctypes.data)
+        if rc:
+            self._raise(rc)
+        return flags[: offs.size - 1].astype(bool)
 
     # ---- replace / stream: host-side glue over find_iter, as in the reference -------------------
     @staticmethod

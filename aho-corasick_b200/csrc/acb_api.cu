@@ -70,6 +70,12 @@ struct Workspace {
   uint8_t* h_stage[2] = {nullptr, nullptr};
   uint64_t h_stage_cap = 0;
   cudaEvent_t stage_ev[2] = {nullptr, nullptr};
+  // batched search: document offsets, per-document counts and their inclusive scan [3][docs_cap], flags [docs_cap]
+  uint64_t* d_docs = nullptr;
+  uint8_t* d_doc_flags = nullptr;
+  uint64_t docs_cap = 0;
+  void* d_temp3 = nullptr;  // scan temp
+  size_t temp3_bytes = 0;
 };
 
 }  // namespace
@@ -157,6 +163,7 @@ void destroy_workspace(Workspace& w) {
   for (int i = 0; i < 2; ++i) { cudaFree(w.d_keys[i]); cudaFree(w.d_pids[i]); }
   cudaFree(w.d_counter); cudaFree(w.d_temp); cudaFree(w.d_hay); cudaFree(w.d_seq);
   cudaFree(w.d_scratch); cudaFree(w.d_flags); cudaFree(w.d_temp2);
+  cudaFree(w.d_docs); cudaFree(w.d_doc_flags); cudaFree(w.d_temp3);
   if (w.h_counter) cudaFreeHost(w.h_counter);
   if (w.h_keys) cudaFreeHost(w.h_keys);
   if (w.h_pids) cudaFreeHost(w.h_pids);
@@ -776,6 +783,21 @@ int ensure_seq(Workspace& w, uint64_t cap) {
   return ACG_OK;
 }
 
+// batched search: room for n entries in each per-document array
+int ensure_docs(Workspace& w, uint64_t n) {
+  if (n <= w.docs_cap) return ACG_OK;
+  cudaFree(w.d_docs);
+  cudaFree(w.d_doc_flags);
+  w.d_docs = nullptr;
+  w.d_doc_flags = nullptr;
+  w.docs_cap = 0;
+  const uint64_t cap = std::max<uint64_t>(n, 1 << 12);
+  CK(cudaMalloc(&w.d_docs, cap * 3 * 8));
+  CK(cudaMalloc(&w.d_doc_flags, cap));
+  w.docs_cap = cap;
+  return ACG_OK;
+}
+
 // enforce_anchored_consistency, src/ahocorasick.rs:2778-2789
 int check_anchored(int have, int want_anchored) {
   if (have == ACG_START_BOTH) return ACG_OK;
@@ -793,6 +815,13 @@ int check_start(const HostDfa& h, int anchored) {
 struct TupleResult {
   uint64_t n = 0;
   int sorted_buf = 0;
+};
+
+// A batched search's documents (device copy of the CSR offsets) as seen by the prefilter engine.
+struct DocBatch {
+  const uint64_t* d_offsets = nullptr;
+  uint64_t n = 0;
+  bool unordered = false;  // is_match: one list, no order step (only the documents of the tuples matter)
 };
 
 // K1 + K4 on a device-resident haystack; leaves `n` ordered tuples in
@@ -908,7 +937,8 @@ BucketPlan plan_buckets(const acg_dfa* a, uint64_t n_bytes) {
 // Enqueue one K3/K3b launch covering the start offsets [scan_lo, scan_hi) of the span.
 int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable,
                             uint64_t span_start, uint64_t span_end, uint64_t scan_lo,
-                            uint64_t scan_hi, int mode, int dev_sms, const BucketPlan& bp) {
+                            uint64_t scan_hi, int mode, int dev_sms, const BucketPlan& bp,
+                            const DocBatch* docs) {
   Workspace& w = cur_ws();
   const PrefilterPlan& pf = a->pf;
   // 16-byte aligned filter region whose 4-byte look-ahead stays inside the readable bytes
@@ -953,6 +983,8 @@ int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t rea
   p.bucket_shift = bp.shift;
   p.bucket_log = bp.log;
   p.bucket_slots = bp.slots();
+  p.doc_offsets = docs ? docs->d_offsets : nullptr;
+  p.n_docs = docs ? docs->n : 0;
   p.bs_n = 0;
   for (int i = 0; i < 3; ++i) { p.bs_needle[i] = 0; p.bs_back[i] = 0; }
   if (pf.bs_n && !a->bytescan_inert && !(a->experiment & ACG_EXP_NO_BYTESCAN)) {
@@ -1126,8 +1158,9 @@ int ensure_stage(Workspace& w, uint64_t bytes) {
 // H2D copy and the scan overlap.
 int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uint64_t span_start,
                   uint64_t span_end, int mode, TupleResult* res, const uint8_t* h_hay = nullptr,
-                  uint64_t scan_lo = UINT64_MAX, uint64_t scan_hi = UINT64_MAX) {
+                  uint64_t scan_lo = UINT64_MAX, uint64_t scan_hi = UINT64_MAX, const DocBatch* docs = nullptr) {
   if (scan_lo == UINT64_MAX) { scan_lo = span_start; scan_hi = span_end; }
+  const bool unordered = docs && docs->unordered;
   Workspace& w = cur_ws();
   const uint64_t n_bytes = span_end - span_start;
   if (n_bytes >= (1ull << (64 - acb::kTieBits))) return ACG_E_INVALID_ARG;
@@ -1137,7 +1170,7 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
   // denser outputs are detected through the counter and the scan is repeated with room
   uint64_t cap = std::max<uint64_t>(w.cap, std::max<uint64_t>(1 << 20, (scan_hi - scan_lo) / 256));
   // bucketed emission: the buckets' slots, then at least 64 K slots of overflow list
-  const BucketPlan bp = plan_buckets(a, n_bytes);
+  const BucketPlan bp = unordered ? BucketPlan{} : plan_buckets(a, n_bytes);
   cap = std::max<uint64_t>(cap, bp.slots() + (bp.shift ? (1u << 16) : 0));
   const size_t counter_bytes = bp.shift ? 8 * (acb::kBucketCountersAt + size_t(bp.n)) : 16;
   bool copied = h_hay == nullptr;
@@ -1148,7 +1181,7 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
     CK(cudaEventRecord(w.ev0, w.stream));
     if (copied) {
       if ((rc = enqueue_prefilter_range(a, d_hay, readable, span_start, span_end, scan_lo, scan_hi, mode,
-                                        dev_sms, bp)))
+                                        dev_sms, bp, docs)))
         return rc;
     } else {
       // chunked H2D on the copy stream; a chunk's start offsets are scanned once the bytes a
@@ -1182,7 +1215,7 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
         const uint64_t upto = c1 == span_end ? span_end : (c1 > scanned + tail ? c1 - tail : scanned);
         if (upto > scanned || c1 == span_end) {
           if ((rc = enqueue_prefilter_range(a, d_hay, c1 == span_end ? readable : c1, span_start, span_end,
-                                            scanned, upto, mode, dev_sms, bp)))
+                                            scanned, upto, mode, dev_sms, bp, docs)))
             return rc;
           scanned = upto;
         }
@@ -1214,6 +1247,12 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
       const uint64_t need = bp.shift ? overflow : want;
       cap = (w.cap - room) + need + need / 8 + 1024;
       continue;
+    }
+    if (unordered) {  // one list in buffer 0, in emission order
+      res->n = want;
+      res->sorted_buf = 0;
+      cur_ws().stats.raw_matches = want;
+      return ACG_OK;
     }
     return order_tuples(a, want, n_bytes, res, bp, overflow);
   }
@@ -1276,9 +1315,12 @@ int run_chain(const acg_dfa* a, int mode, TupleResult* r) {
   return ACG_OK;
 }
 
-// D2H + expansion of ordered (key,pid) tuples into acg_match / count / fnv.
+// D2H + expansion of ordered (key,pid) tuples into acg_match / count / fnv.  Batched search (`docs`,
+// the host CSR offsets): acg_doc_match records -- the document in the pad, offsets relative to it.  No
+// match crosses a document end, so the ordered tuples are document-major and one forward walk over the
+// offsets tags them.
 int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, acg_match* out,
-                 uint64_t cap, uint64_t* n_out, uint64_t* fnv, int key_mode = 0) {
+                 uint64_t cap, uint64_t* n_out, uint64_t* fnv, int key_mode = 0, const uint64_t* docs = nullptr) {
   Workspace& w = cur_ws();
   *n_out = r.n;
   if (fnv) *fnv = 0xcbf29ce484222325ull;
@@ -1299,6 +1341,7 @@ int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, ac
   auto mix = [&](uint64_t v) {
     for (int k = 0; k < 8; ++k) { hsh ^= (v >> (8 * k)) & 0xFF; hsh *= 0x100000001b3ull; }
   };
+  uint32_t doc = 0;
   for (uint64_t i = 0; i < r.n; ++i) {
     const uint32_t pid = w.h_pids[i];
     uint64_t start, end;
@@ -1309,9 +1352,14 @@ int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, ac
       end = span_start + (w.h_keys[i] >> acb::kTieBits);
       start = end - plens[pid];
     }
+    if (docs) {
+      while (docs[doc + 1] <= start) ++doc;
+      start -= docs[doc];
+      end -= docs[doc];
+    }
     if (out && i < cap) {
       out[i].pid = pid;
-      out[i]._pad = 0;
+      out[i]._pad = doc;
       out[i].start = start;
       out[i].end = end;
     }
@@ -1704,6 +1752,147 @@ int find_iter_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uin
   return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, mode);
 }
 
+enum BatchKind { kBatchFindIter = 0, kBatchOverlapping = 1, kBatchIsMatch = 2 };
+
+// acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch (include/acb200.h).
+int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
+               const uint64_t* offs, uint64_t n_docs, int anchored, acg_match* out, uint64_t cap, uint64_t* n_out,
+               uint8_t* flags) {
+  if (!a || !offs || (what == kBatchIsMatch ? (!flags && n_docs) : !n_out)) return ACG_E_INVALID_ARG;
+  if (n_out) *n_out = 0;
+  if (n_docs >= (1ull << 32)) return ACG_E_INVALID_ARG;
+  for (uint64_t i = 0; i < n_docs; ++i)
+    if (offs[i + 1] < offs[i]) return ACG_E_INVALID_SPAN;
+  if (offs[n_docs] > hay_len) return ACG_E_INVALID_SPAN;
+  int rc = check_anchored(a->h.start_kind, anchored);
+  if (rc) return rc;
+  if (what == kBatchOverlapping) {  // Automaton::try_find_overlapping_iter, src/automaton.rs:397-423
+    if (a->h.match_kind != ACG_STANDARD) return ACG_E_UNSUPPORTED_OVERLAPPING;
+    if (anchored) return ACG_E_INVALID_INPUT_ANCHORED;
+  }
+  if ((rc = check_start(a->h, anchored))) return rc;
+  if (!a->on_device) return ACG_E_NO_DEVICE;
+  if (n_docs == 0) return ACG_OK;
+  const int engine = a->engine_override;
+  if (engine == ACG_ENGINE_PREFILTER && (!a->pf.supported || anchored)) return ACG_E_INVALID_ARG;
+  const bool use_pf = engine != ACG_ENGINE_SEQUENTIAL && a->pf.supported && !anchored;
+  DeviceGuard guard(a->device);
+  WsLease lease(a);
+  if (lease.rc) return lease.rc;
+  Workspace& w = cur_ws();
+  w.stats.engine = use_pf ? ACG_ENGINE_PREFILTER : ACG_ENGINE_SEQUENTIAL;
+  const uint64_t span_start = offs[0], span_end = offs[n_docs], nd1 = n_docs + 1;
+  if ((rc = ensure_docs(w, nd1))) return rc;
+  uint64_t* d_offs = w.d_docs;
+  unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(w.d_docs + w.docs_cap);
+  unsigned long long* d_incl = d_counts + w.docs_cap;
+  CK(cudaMemcpyAsync(d_offs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
+  const uint8_t* d_base = hay;
+  uint64_t readable = hay_len;
+  const bool pipelined = !hay_on_device && use_pf;
+  if (!hay_on_device) {
+    if ((rc = stage_host_span(a, hay, span_start, span_end, &d_base, pipelined))) return rc;
+    readable = span_end + 32;
+  }
+  auto fetch_flags = [&]() -> int {
+    CK(cudaMemcpyAsync(flags, w.d_doc_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    return ACG_OK;
+  };
+  float ms = 0;
+  if (!use_pf) {
+    // one thread per document: count, inclusive scan, fill at each document's offset
+    acb::SeqDocsLaunch p{};
+    p.hay = d_base;
+    p.doc_offsets = d_offs;
+    p.n_docs = n_docs;
+    p.anchored = anchored;
+    p.match_kind = a->h.match_kind;
+    p.overlapping = what == kBatchOverlapping;
+    p.single = what == kBatchIsMatch;
+    CK(cudaEventRecord(w.ev0, w.stream));
+    if (what == kBatchIsMatch) {
+      p.flags = w.d_doc_flags;
+      CK(acb::launch_seq_docs(a->dev, p, w.stream));
+      CK(cudaEventRecord(w.ev1, w.stream));
+      if ((rc = fetch_flags())) return rc;
+      cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+      w.stats.scan_ms = ms;
+      w.stats.launches += 1;
+      return ACG_OK;
+    }
+    p.counts = d_counts;
+    CK(acb::launch_seq_docs(a->dev, p, w.stream));
+    size_t tb = 0;
+    CK(acb::inclusive_sum_u64(nullptr, tb, d_counts, d_incl, n_docs, w.stream));
+    if (tb > w.temp3_bytes) {
+      cudaFree(w.d_temp3);
+      w.d_temp3 = nullptr;
+      w.temp3_bytes = 0;
+      CK(cudaMalloc(&w.d_temp3, tb));
+      w.temp3_bytes = tb;
+    }
+    tb = w.temp3_bytes;
+    CK(acb::inclusive_sum_u64(w.d_temp3, tb, d_counts, d_incl, n_docs, w.stream));
+    CK(cudaMemcpyAsync(w.h_counter, d_incl + n_docs - 1, 8, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    const uint64_t total = w.h_counter[0];
+    *n_out = total;
+    w.stats.raw_matches = total;
+    w.stats.launches += 2;
+    if (total > cap) return ACG_E_OVERFLOW;
+    if (total) {
+      if (!out) return ACG_E_INVALID_ARG;
+      if ((rc = ensure_seq(w, total))) return rc;
+      p.incl = d_incl;
+      p.out = w.d_seq;
+      p.cap = total;
+      CK(acb::launch_seq_docs(a->dev, p, w.stream));
+      w.stats.launches += 1;
+    }
+    CK(cudaEventRecord(w.ev1, w.stream));
+    if (total) CK(cudaMemcpyAsync(out, w.d_seq, total * 24, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+    w.stats.scan_ms = ms;
+    return ACG_OK;
+  }
+  // prefilter engine over the whole span, each match bounded by its document (PrefilterLaunch::doc_offsets)
+  const int chain_mode = what == kBatchOverlapping || a->h.match_kind == ACG_STANDARD ? 0 : 1;
+  const int pf_mode = what == kBatchOverlapping ? 0 : (chain_mode == 0 ? 2 : 1);
+  DocBatch docs;
+  docs.d_offsets = d_offs;
+  docs.n = n_docs;
+  docs.unordered = what == kBatchIsMatch;
+  TupleResult r;
+  if ((rc = run_prefilter(a, d_base, readable, span_start, span_end, pf_mode, &r, pipelined ? hay : nullptr,
+                          UINT64_MAX, UINT64_MAX, &docs)))
+    return rc;
+  if (what == kBatchIsMatch) {
+    acb::DocFlagsLaunch f;
+    f.keys = w.d_keys[r.sorted_buf];
+    f.pids = w.d_pids[r.sorted_buf];
+    f.pattern_lens = a->d_plens;
+    f.n = r.n;
+    f.mode = chain_mode;
+    f.span_start = span_start;
+    f.doc_offsets = d_offs;
+    f.n_docs = n_docs;
+    f.flags = w.d_doc_flags;
+    CK(cudaEventRecord(w.ev2, w.stream));
+    CK(cudaMemsetAsync(w.d_doc_flags, 0, n_docs, w.stream));
+    CK(acb::launch_doc_flags(f, w.stream));
+    CK(cudaEventRecord(w.ev3, w.stream));
+    if ((rc = fetch_flags())) return rc;
+    cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+    w.stats.order_ms = ms;
+    w.stats.launches += 1;
+    return ACG_OK;
+  }
+  if (what == kBatchFindIter && (rc = run_chain(a, chain_mode, &r))) return rc;
+  return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, chain_mode, offs);
+}
+
 }  // namespace
 
 extern "C" {
@@ -2036,6 +2225,24 @@ int acg_find_iter_dev(const acg_dfa* a, const void* d_hay, uint64_t hay_len, uin
                       float* kernel_ms) {
   return find_iter_impl(a, static_cast<const uint8_t*>(d_hay), true, hay_len, span_start, span_end, 0,
                         out, cap, n_out, kernel_ms);
+}
+
+int acg_find_iter_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                        const uint64_t* doc_offsets, uint64_t n_docs, int anchored, acg_doc_match* out, uint64_t cap,
+                        uint64_t* n_out) {
+  return batch_impl(a, kBatchFindIter, hay, hay_on_device != 0, hay_len, doc_offsets, n_docs, anchored,
+                    reinterpret_cast<acg_match*>(out), cap, n_out, nullptr);
+}
+int acg_find_overlapping_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                               const uint64_t* doc_offsets, uint64_t n_docs, int anchored, acg_doc_match* out,
+                               uint64_t cap, uint64_t* n_out) {
+  return batch_impl(a, kBatchOverlapping, hay, hay_on_device != 0, hay_len, doc_offsets, n_docs, anchored,
+                    reinterpret_cast<acg_match*>(out), cap, n_out, nullptr);
+}
+int acg_is_match_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                       const uint64_t* doc_offsets, uint64_t n_docs, int anchored, uint8_t* flags) {
+  return batch_impl(a, kBatchIsMatch, hay, hay_on_device != 0, hay_len, doc_offsets, n_docs, anchored, nullptr, 0,
+                    nullptr, flags);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

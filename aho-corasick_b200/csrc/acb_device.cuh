@@ -89,6 +89,43 @@ struct SeqLaunch {
 };
 cudaError_t launch_seq_find(const DfaDev& dfa, const SeqLaunch& p, cudaStream_t s);
 
+// The same engine over a batch of documents, one thread per document (acg_*_batch when the
+// prefilter engine does not apply).  Two launches: the count pass (incl == nullptr) fills
+// counts[n_docs] -- or flags[n_docs] for is_match -- and after an inclusive scan of the counts the fill
+// pass writes each document's records at out[incl[doc - 1] * 3] as (pid | doc << 32, start, end) with
+// offsets relative to the document, the acg_doc_match layout.  A long document is one thread's walk.
+struct SeqDocsLaunch {
+  const uint8_t* hay;
+  const uint64_t* doc_offsets;  // [n_docs + 1], haystack offsets
+  uint64_t n_docs;
+  int anchored;
+  int match_kind;
+  int overlapping;              // 1: find_overlapping_iter, 0: find_iter
+  int single;                   // 1: stop at the first match (is_match)
+  unsigned long long* counts;   // count pass: [n_docs]
+  uint8_t* flags;               // count pass, is_match: [n_docs] instead of counts
+  const unsigned long long* incl;   // fill pass: [n_docs] inclusive scan of counts
+  uint64_t* out;
+  uint64_t cap;                 // records
+};
+cudaError_t launch_seq_docs(const DfaDev& dfa, const SeqDocsLaunch& p, cudaStream_t s);
+cudaError_t inclusive_sum_u64(void* d_temp, size_t& temp_bytes, const unsigned long long* in, unsigned long long* out,
+                              uint64_t n, cudaStream_t s);
+
+// is_match over a batch on the prefilter engine: flags[doc] = 1 for the document of each of n tuples.
+struct DocFlagsLaunch {
+  const uint64_t* keys;
+  const uint32_t* pids;
+  const uint32_t* pattern_lens;
+  uint64_t n;
+  int mode;                     // key layout as ChainLaunch::mode
+  uint64_t span_start;
+  const uint64_t* doc_offsets;  // [n_docs + 1]
+  uint64_t n_docs;
+  uint8_t* flags;
+};
+cudaError_t launch_doc_flags(const DocFlagsLaunch& f, cudaStream_t s);
+
 // K3/K3b: position-parallel k-gram prefilter fused with the anchored DFA verify.
 // Plays the role of the reference's packed/Teddy prefilter (src/packed/teddy/
 // generic.rs:114-713 candidate + :820-870 verify): a cheap per-position
@@ -142,6 +179,10 @@ struct PrefilterLaunch {
   uint32_t bucket_shift;
   uint32_t bucket_log;
   uint64_t bucket_slots;        // n_buckets << bucket_log
+  // Batched search (acg_*_batch): CSR document bounds in haystack offsets, [n_docs + 1] on the device; a match is
+  // reported only if it ends inside the document its start lies in.  nullptr / 0: one haystack.
+  const uint64_t* doc_offsets;
+  uint64_t n_docs;
 };
 cudaError_t launch_prefilter(const DfaDev& dfa, const PrefilterLaunch& p, int sm_count, cudaStream_t s);
 cudaError_t launch_bytescan(const DfaDev& dfa, const PrefilterLaunch& p, int sm_count, cudaStream_t s);

@@ -6,6 +6,7 @@
 //                                 (src/dfa.rs:218-226) + match expansion (:275-286)
 //   Kseq seq_find_kernel          single-lane FindIter/try_find (anchored inputs,
 //                                 empty-pattern automata)
+//        seq_docs_kernel          the same per document of a batch, one thread each
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
 #ifndef ACB_PTX_HEADER
@@ -18,6 +19,7 @@
 #include <cstdlib>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 namespace acb {
 
@@ -157,7 +159,7 @@ __device__ __forceinline__ SeqMatch seq_get_match(const DfaDev& d, uint32_t sid,
 }
 
 // try_find_fwd_imp, src/automaton.rs:1285-1420 (prefilter-free instance)
-__device__ bool seq_try_find(const DfaDev& d, const uint8_t* hay, uint64_t start, uint64_t end,
+__device__ __forceinline__ bool seq_try_find(const DfaDev& d, const uint8_t* hay, uint64_t start, uint64_t end,
                              bool anchored, bool earliest, SeqMatch* out) {
   if (start > end) return false;
   uint32_t sid = anchored ? d.start_anchored_id : d.start_unanchored_id;
@@ -186,34 +188,116 @@ __device__ bool seq_try_find(const DfaDev& d, const uint8_t* hay, uint64_t start
   return have;
 }
 
-__global__ void seq_find_kernel(DfaDev d, SeqLaunch p) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const bool anchored = p.anchored != 0;
-  const bool earliest = p.match_kind == 0 || p.earliest != 0;
-  uint64_t start = p.span_start;
+// FindIter (src/automaton.rs:857-936) over [span_start, span_end): writes the i-th match as
+// (pid | tag, start - base, end - base) at out[(first + i) * 3] while first + i < cap (out may be
+// null: count only) and returns the number of matches.
+__device__ __forceinline__ unsigned long long seq_find_iter(const DfaDev& d, const uint8_t* hay, uint64_t span_start, uint64_t span_end,
+                                            bool anchored, bool earliest, bool single, uint64_t* out,
+                                            unsigned long long first, uint64_t cap, uint64_t tag, uint64_t base) {
+  uint64_t start = span_start;
   unsigned long long n = 0;
   bool have_last = false;
   uint64_t last_end = 0;
   for (;;) {
     SeqMatch m;
-    if (!seq_try_find(d, p.hay, start, p.span_end, anchored, earliest, &m)) break;
-    if (!p.single && m.start == m.end && have_last && m.end == last_end) {
+    if (!seq_try_find(d, hay, start, span_end, anchored, earliest, &m)) break;
+    if (!single && m.start == m.end && have_last && m.end == last_end) {
       // FindIter::handle_overlapping_empty_match, src/automaton.rs:910-920
       start += 1;
-      if (!seq_try_find(d, p.hay, start, p.span_end, anchored, earliest, &m)) break;
+      if (!seq_try_find(d, hay, start, span_end, anchored, earliest, &m)) break;
     }
-    if (n < p.cap) {
-      p.out[n * 3 + 0] = m.pid;
-      p.out[n * 3 + 1] = m.start;
-      p.out[n * 3 + 2] = m.end;
+    if (out && first + n < cap) {
+      out[(first + n) * 3 + 0] = m.pid | tag;
+      out[(first + n) * 3 + 1] = m.start - base;
+      out[(first + n) * 3 + 2] = m.end - base;
     }
     ++n;
-    if (p.single) break;
+    if (single) break;
     start = m.end;
     last_end = m.end;
     have_last = true;
   }
-  *p.counter = n;
+  return n;
+}
+
+// try_find_overlapping_fwd_imp (src/automaton.rs:1443-1537) run to the end of [lo, hi), unanchored:
+// the start state's matches at lo, then every list entry of each match state entered, in list order.
+// Same output convention as seq_find_iter.
+__device__ __forceinline__ unsigned long long seq_overlapping(const DfaDev& d, const uint8_t* hay, uint64_t lo, uint64_t hi,
+                                              uint64_t* out, unsigned long long first, uint64_t cap, uint64_t tag) {
+  unsigned long long n = 0;
+  uint32_t sid = d.start_unanchored_id;
+  bool report = seq_is_match(d, sid);  // the start state's matches end at lo
+  for (uint64_t at = lo;;) {           // `at`: end offset of the matches of sid
+    if (report) {
+      const uint32_t row = (sid >> d.stride2) - 2;
+      for (uint32_t i = d.match_offsets[row]; i < d.match_offsets[row + 1]; ++i, ++n) {
+        if (!out || first + n >= cap) continue;
+        const uint32_t pid = d.match_pids[i];
+        out[(first + n) * 3 + 0] = pid | tag;
+        out[(first + n) * 3 + 1] = at - d.pattern_lens[pid] - lo;
+        out[(first + n) * 3 + 2] = at - lo;
+      }
+    }
+    if (at >= hi) break;
+    sid = d.trans[sid + d.classes[hay[at]]];
+    ++at;
+    if (sid == 0) break;  // DEAD
+    report = sid <= d.max_match_id;
+  }
+  return n;
+}
+
+__global__ void seq_find_kernel(DfaDev d, SeqLaunch p) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  const bool earliest = p.match_kind == 0 || p.earliest != 0;
+  *p.counter = seq_find_iter(d, p.hay, p.span_start, p.span_end, p.anchored != 0, earliest, p.single != 0, p.out, 0,
+                             p.cap, 0, 0);
+}
+
+struct SumOp {
+  __device__ __forceinline__ unsigned long long operator()(unsigned long long a, unsigned long long b) const { return a + b; }
+};
+
+// One thread per document of a batch.  Count pass (incl == nullptr): counts[doc] = its number of
+// matches, or flags[doc] = (a match exists) when flags is given.  Fill pass: the document's records from
+// index incl[doc - 1] (the matches of the documents before it) on, tagged with the document
+// (doc << 32 in the pid word, offsets relative to the document's first byte).
+constexpr int kSeqDocThreads = 128;
+template <bool OVERLAPPING>
+__global__ void __launch_bounds__(kSeqDocThreads) seq_docs_kernel(DfaDev d, SeqDocsLaunch p) {
+  const uint64_t doc = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (doc >= p.n_docs) return;
+  const uint64_t lo = p.doc_offsets[doc], hi = p.doc_offsets[doc + 1];
+  const bool fill = p.incl != nullptr;
+  uint64_t* out = fill ? p.out : nullptr;
+  const unsigned long long first = fill && doc ? p.incl[doc - 1] : 0;
+  const uint64_t tag = doc << 32;
+  unsigned long long n;
+  if constexpr (OVERLAPPING) {
+    n = seq_overlapping(d, p.hay, lo, hi, out, first, p.cap, tag);
+  } else {
+    const bool earliest = p.match_kind == 0 || p.single != 0;
+    n = seq_find_iter(d, p.hay, lo, hi, p.anchored != 0, earliest, p.single != 0, out, first, p.cap, tag, lo);
+  }
+  if (fill) return;
+  if (p.flags) p.flags[doc] = n != 0;
+  else p.counts[doc] = n;
+}
+
+// is_match over a batch, prefilter engine: flags[doc] = 1 for the document of every tuple (key as
+// ChainLaunch::mode: 1 = start_rel << 24 | len, 0 = end_rel << 24 | tie).
+__global__ void doc_flags_kernel(DocFlagsLaunch f) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= f.n) return;
+  const uint64_t key = f.keys[i];
+  const uint64_t s = f.span_start + (f.mode == 1 ? key >> kTieBits : (key >> kTieBits) - f.pattern_lens[f.pids[i]]);
+  uint64_t lo = 1, hi = f.n_docs;  // the first document end past s
+  while (lo < hi) {
+    const uint64_t mid = lo + ((hi - lo) >> 1);
+    if (f.doc_offsets[mid] > s) hi = mid; else lo = mid + 1;
+  }
+  f.flags[lo - 1] = 1;
 }
 
 // Records built in shared memory and stored as 16-byte vectors: the target may be another GPU's HBM
@@ -303,6 +387,25 @@ cudaError_t launch_dfa_fill_level(const FillLaunch& f, cudaStream_t s) {
 cudaError_t launch_seq_find(const DfaDev& dfa, const SeqLaunch& p, cudaStream_t s) {
   ACB_LAUNCH(seq_find_kernel, 1, 32, 0, s, dfa, p);
   return cudaGetLastError();
+}
+
+cudaError_t launch_seq_docs(const DfaDev& dfa, const SeqDocsLaunch& p, cudaStream_t s) {
+  if (p.n_docs == 0) return cudaSuccess;
+  const unsigned blocks = (unsigned)((p.n_docs + kSeqDocThreads - 1) / kSeqDocThreads);
+  if (p.overlapping) ACB_LAUNCH(seq_docs_kernel<true>, blocks, kSeqDocThreads, 0, s, dfa, p);
+  else ACB_LAUNCH(seq_docs_kernel<false>, blocks, kSeqDocThreads, 0, s, dfa, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_doc_flags(const DocFlagsLaunch& f, cudaStream_t s) {
+  if (f.n == 0) return cudaSuccess;
+  ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
+  return cudaGetLastError();
+}
+
+cudaError_t inclusive_sum_u64(void* d_temp, size_t& temp_bytes, const unsigned long long* in, unsigned long long* out,
+                              uint64_t n, cudaStream_t s) {
+  return cub::DeviceScan::InclusiveScan(d_temp, temp_bytes, in, out, SumOp(), (int64_t)n, s);
 }
 
 cudaError_t sort_pairs(void* d_temp, size_t& temp_bytes, const uint64_t* keys_in, uint64_t* keys_out,

@@ -182,9 +182,25 @@ __device__ __forceinline__ uint32_t anchor_lookup_key(const DfaDev& d, uint32_t 
   }
 }
 
+// Batched search: the end of the document that contains start offset s, i.e. doc_offsets[i] for the
+// first i with doc_offsets[i] > s (the span is [doc_offsets[0], doc_offsets[n_docs]), so i exists).
+// Only candidates that reach a match state pay for it.  (Out of line, the call makes ptxas spill
+// around it in every prefilter_kernel instantiation.)
+__device__ __forceinline__ uint64_t doc_end_of(const uint64_t* __restrict__ offs, uint64_t n_docs, uint64_t s) {
+  uint64_t lo = 1, hi = n_docs;  // answer in [1, n_docs]
+  while (lo < hi) {
+    const uint64_t mid = lo + ((hi - lo) >> 1);
+    if (__ldg(offs + mid) > s) hi = mid; else lo = mid + 1;
+  }
+  return __ldg(offs + lo);
+}
+
 // Verify one candidate start offset `s` (K3b): walk the shipped DFA while the state stays on the
 // trie path anchored at s (depth == bytes consumed), starting from state `sid` at depth `j`
 // (the start state, or the state the anchor map gave for the first j bytes).
+// Batched search (p.doc_offsets): a match must end inside the document s lies in; the walk stops at
+// the first match state past that end (any longer match ends later still).  The end is looked up at
+// each match state the walk reaches (most candidates that match reach one).
 template <int MODE, class EM>
 __device__ __forceinline__ void verify_from(const DfaDev& d, const PrefilterLaunch& p, const uint8_t* s_cls,
                                             uint64_t s, uint32_t sid, uint32_t j, EM& em) {
@@ -205,6 +221,8 @@ __device__ __forceinline__ void verify_from(const DfaDev& d, const PrefilterLaun
     }
     entered = false;
     if (sid <= d.max_match_id) {
+      // (no end cached across the loop: a live 64-bit value there costs the single-haystack scans)
+      if (p.doc_offsets != nullptr && pos > doc_end_of(p.doc_offsets, p.n_docs, s)) break;
       const uint32_t row = sid >> d.stride2;
       const uint32_t lo = __ldg(d.match_offsets + row - 2), hi = __ldg(d.match_offsets + row - 1);
       if (MODE == 0) {

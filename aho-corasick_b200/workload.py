@@ -124,6 +124,20 @@ CONFIGS = {
 }
 
 
+def doc_offsets(n_bytes: int, seed: int, lo: int = 16, hi: int = 16384) -> np.ndarray:
+    """CSR bounds (int64, [n_docs + 1]) cutting [0, n_bytes) into documents whose lengths are log-uniform
+    in [lo, hi] (the last one is cut short); mean (hi - lo) / ln(hi / lo), about 2.3 KiB by default."""
+    rng = np.random.default_rng(seed)
+    mean = (hi - lo) / np.log(hi / lo)
+    lens = np.exp(rng.uniform(np.log(lo), np.log(hi + 1), size=int(n_bytes / mean * 1.1) + 16)).astype(np.int64)
+    ends = np.cumsum(lens)
+    while ends[-1] < n_bytes:  # (not reached for sizes above a few MiB)
+        more = np.exp(rng.uniform(np.log(lo), np.log(hi + 1), size=1024)).astype(np.int64)
+        ends = np.concatenate([ends, ends[-1] + np.cumsum(more)])
+    k = int(np.searchsorted(ends, n_bytes))
+    return np.concatenate([[0], ends[:k], [n_bytes]]).astype(np.int64)
+
+
 def config_patterns(name: str):
     """The pattern set of a named configuration."""
     c = CONFIGS[name]

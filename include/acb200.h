@@ -191,6 +191,36 @@ int acg_count_overlapping_dev(const acg_dfa* dfa, const void* d_hay, uint64_t ha
                               uint64_t span_start, uint64_t span_end,
                               uint64_t* n_out, uint64_t* fnv, float* kernel_ms);
 
+/* ---- batched search: many independent documents in one call -----------------
+ * A batch is one byte buffer plus CSR offsets doc_offsets[n_docs + 1] (host memory, non-decreasing,
+ * doc_offsets[n_docs] <= hay_len); document d is hay[doc_offsets[d] .. doc_offsets[d + 1]), empty
+ * documents allowed.  For every d, the records tagged doc == d are exactly what the single-haystack
+ * call returns on that document alone -- same (pid, start, end), offsets relative to the document's
+ * first byte, same order -- and the records appear in ascending d.  Error codes are those of the
+ * single calls; decreasing offsets or offsets past hay_len give ACG_E_INVALID_SPAN, n_docs >= 2^32
+ * ACG_E_INVALID_ARG.  hay_on_device != 0: `hay` is a device pointer to byte 0.  Results go to host
+ * memory; two-call protocol on ACG_E_OVERFLOW (*n_out holds the required count).
+ * Engine: the prefilter engine when the automaton has a prefilter plan and the input is unanchored,
+ * else (and with ACG_ENGINE_SEQUENTIAL) one thread per document running the reference's loop --
+ * a single very long document is then one thread's sequential walk. */
+typedef struct {
+  uint32_t pid;
+  uint32_t doc; /* acg_match layout, the document index in the pad */
+  uint64_t start;
+  uint64_t end;
+} acg_doc_match;
+/* AhoCorasick::try_find_iter(doc) for every document */
+int acg_find_iter_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                        const uint64_t* doc_offsets, uint64_t n_docs, int anchored,
+                        acg_doc_match* out, uint64_t cap, uint64_t* n_out);
+/* AhoCorasick::try_find_overlapping_iter(doc) for every document */
+int acg_find_overlapping_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                               const uint64_t* doc_offsets, uint64_t n_docs, int anchored,
+                               acg_doc_match* out, uint64_t cap, uint64_t* n_out);
+/* AhoCorasick::is_match(doc) for every document: flags[d] = 0 / 1 */
+int acg_is_match_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                       const uint64_t* doc_offsets, uint64_t n_docs, int anchored, uint8_t* flags);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

@@ -296,6 +296,40 @@ class AhoCorasick {
   }
   void find_overlapping(const Input& in, OverlappingState& state) const { try_find_overlapping(in, state).unwrap(); }  // :470
 
+  // Batched search (acg_*_batch, include/acb200.h): many documents in one device call.  `offsets` are the
+  // CSR bounds [n_docs + 1] into `haystack`; per document the result is the single-haystack call's on that
+  // document alone, offsets relative to it.
+  using PerDoc = std::vector<std::vector<Match>>;
+  Result<PerDoc> try_find_iter_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                     Anchored a = Anchored::No) const {
+    return collect_batch(acg_find_iter_batch, haystack, offsets, a);
+  }
+  Result<PerDoc> try_find_overlapping_iter_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                                 Anchored a = Anchored::No) const {
+    return collect_batch(acg_find_overlapping_batch, haystack, offsets, a);
+  }
+  Result<std::vector<bool>> try_is_match_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                               Anchored a = Anchored::No) const {
+    Result<std::vector<bool>> r;
+    if (offsets.empty()) { r.error = ACG_E_INVALID_ARG; return r; }
+    std::vector<uint8_t> flags(offsets.size());
+    r.error = acg_is_match_batch(h_, reinterpret_cast<const uint8_t*>(haystack.data()), 0, haystack.size(),
+                                 offsets.data(), offsets.size() - 1, int(a), flags.data());
+    if (r.error == 0) r.value.assign(flags.begin(), flags.end() - 1);
+    return r;
+  }
+  PerDoc find_iter_batch(std::string_view haystack, const std::vector<uint64_t>& offsets, Anchored a = Anchored::No) const {
+    return std::move(try_find_iter_batch(haystack, offsets, a).unwrap());
+  }
+  PerDoc find_overlapping_iter_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                     Anchored a = Anchored::No) const {
+    return std::move(try_find_overlapping_iter_batch(haystack, offsets, a).unwrap());
+  }
+  std::vector<bool> is_match_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                   Anchored a = Anchored::No) const {
+    return std::move(try_is_match_batch(haystack, offsets, a).unwrap());
+  }
+
   // replace_all_with / replace_all_with_bytes, :834 / :887 (src/automaton.rs:498-550)
   template <class F>
   void replace_all_with(std::string_view haystack, std::string& dst, F&& replace_with) const {
@@ -363,6 +397,31 @@ class AhoCorasick {
       out.reserve(n);
       for (uint64_t i = 0; i < n; ++i) out.emplace_back(buf[i].pid, buf[i].start, buf[i].end);
       r.value = MatchIter(std::move(out));
+    }
+    return r;
+  }
+  using BatchFn = int (*)(const acg_dfa*, const uint8_t*, int, uint64_t, const uint64_t*, uint64_t, int, acg_doc_match*,
+                          uint64_t, uint64_t*);
+  Result<PerDoc> collect_batch(BatchFn fn, std::string_view haystack, const std::vector<uint64_t>& offsets, Anchored a) const {
+    Result<PerDoc> r;
+    if (offsets.empty()) { r.error = ACG_E_INVALID_ARG; return r; }
+    const uint64_t n_docs = offsets.size() - 1;
+    std::vector<acg_doc_match> buf(std::max<uint64_t>(cap_hint_, haystack.size() / 256 + 64));
+    uint64_t n = 0;
+    for (;;) {
+      const int rc = fn(h_, reinterpret_cast<const uint8_t*>(haystack.data()), 0, haystack.size(), offsets.data(), n_docs,
+                        int(a), buf.data(), buf.size(), &n);
+      if (rc == ACG_E_OVERFLOW) {
+        cap_hint_ = n + n / 8 + 64;
+        buf.resize(cap_hint_);
+        continue;
+      }
+      r.error = rc;
+      break;
+    }
+    if (r.error == 0) {
+      r.value.resize(n_docs);
+      for (uint64_t i = 0; i < n; ++i) r.value[buf[i].doc].emplace_back(buf[i].pid, buf[i].start, buf[i].end);
     }
     return r;
   }

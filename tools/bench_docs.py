@@ -1,0 +1,128 @@
+#!/usr/bin/env python3
+"""Batched search over many documents in one device call (acg_find_overlapping_batch).
+
+    python tools/bench_docs.py [--hay-gib 4] [--steps 20] [--warmup 5] [--engine 0]
+
+cfg 2's automaton and haystack (same seeds as bench.py), device-resident, cut at seeded boundaries into
+documents of log-uniform length in [16 B, 16 KiB] (~1.8 M documents, mean ~2.4 KiB at 4 GiB).  Prints one
+JSON line: GiB/s of the batch call's scan + order (CUDA events inside the library), the match count, the
+card's name and power limit, and two checks outside the timed region:
+  * mapped back to global offsets, the batch list is cfg 2's single-haystack list minus the matches that
+    straddle a document boundary, record for record (count and FNV-1a reported);
+  * call overhead on the first 10 000 documents: one single-haystack call per document against one batch
+    call over the same documents (same match count).
+"""
+import argparse
+import importlib.util
+import json
+import sys
+import time
+from pathlib import Path
+
+ROOT = Path(__file__).resolve().parents[1]
+sys.path.insert(0, str(ROOT))
+sys.dont_write_bytecode = True
+GIB = float(1 << 30)
+
+
+def clock_sampler():
+    """bench.py's ClockSampler (card name, power limit, SM clocks during the timed steps)."""
+    spec = importlib.util.spec_from_file_location("acb_bench", ROOT / "bench.py")
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod.ClockSampler
+
+
+def fnv1a(rec):
+    """FNV-1a 64 over the little-endian (pid, start, end) u64 stream of match records, as
+    acg_count_overlapping_dev computes it (a byte-serial loop: a few seconds for a million records)."""
+    import numpy as np
+    words = np.empty((len(rec), 3), np.uint64)
+    words[:, 0], words[:, 1], words[:, 2] = rec["pid"], rec["start"], rec["end"]
+    h, prime, mask = 0xcbf29ce484222325, 0x100000001b3, (1 << 64) - 1
+    for b in words.reshape(-1).view(np.uint8).tobytes():
+        h = ((h ^ b) * prime) & mask
+    return h
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--hay-gib", type=float, default=4.0)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--engine", type=int, default=0, help="0 auto, 3 the per-document sequential kernel")
+    args = ap.parse_args()
+    import numpy as np
+    import torch
+    import aho_corasick_b200 as ab
+    from aho_corasick_b200 import workload as W
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    ClockSampler = clock_sampler()
+    n = int(args.hay_gib * GIB)
+    n -= n % 4096
+    pats = W.config_patterns("cfg2")
+    ac = ab.AhoCorasick.builder().kind(ab.AhoCorasickKind.DFA).build(pats).set_engine(args.engine)
+    d_hay = torch.empty(n, dtype=torch.uint8, device="cuda")
+    W.torch_fill_config("cfg2", d_hay, pats)
+    torch.cuda.synchronize()
+    offs = W.doc_offsets(n, 0xD0C5)
+    batch = (d_hay, offs)
+    for _ in range(args.warmup):
+        got = ac.find_overlapping_iter_batch_np(batch)
+    kernel_ms, scan_ms, order_ms = [], [], []
+    with ClockSampler(0) as clocks:
+        t0 = time.perf_counter()
+        for _ in range(args.steps):
+            got = ac.find_overlapping_iter_batch_np(batch)
+            st = ac.last_stats()
+            kernel_ms.append(st["scan_ms"] + st["order_ms"])
+            scan_ms.append(st["scan_ms"])
+            order_ms.append(st["order_ms"])
+        wall = time.perf_counter() - t0
+    engine = int(ac.last_stats()["engine"])
+    ac.set_engine(ab.Engine.Auto)
+    single, _ = ac.find_overlapping_iter_dev_np(d_hay.data_ptr(), n)
+    doc = np.searchsorted(offs, single["start"].astype(np.int64), side="right") - 1
+    keep = single["end"].astype(np.int64) <= offs[doc + 1]
+    want = single[keep]
+    base = offs[got["doc"].astype(np.int64)].astype(np.uint64)
+    mine = np.empty(len(got), ab.MATCH_DTYPE)
+    mine["pid"], mine["_pad"], mine["start"], mine["end"] = got["pid"], 0, got["start"] + base, got["end"] + base
+    assert len(mine) == len(want) and mine.tobytes() == want.tobytes(), (len(mine), len(want))
+    fnv = fnv1a(mine)
+    k = min(10_000, offs.size - 1)
+    sub = offs[: k + 1]
+    ptr = d_hay.data_ptr()
+    for d in range(min(k, 100)):  # warm
+        ac.find_overlapping_iter_dev_np(ptr, n, span=(int(sub[d]), int(sub[d + 1])))
+    t0 = time.perf_counter()
+    per_doc_n = 0
+    for d in range(k):
+        per_doc_n += len(ac.find_overlapping_iter_dev_np(ptr, n, span=(int(sub[d]), int(sub[d + 1])))[0])
+    per_doc_s = time.perf_counter() - t0
+    ac.find_overlapping_iter_batch_np((d_hay, sub))
+    t0 = time.perf_counter()
+    batch_n = len(ac.find_overlapping_iter_batch_np((d_hay, sub)))
+    batch_s = time.perf_counter() - t0
+    assert batch_n == per_doc_n, (batch_n, per_doc_n)
+    dev_s = sum(kernel_ms) / 1e3
+    print(json.dumps({
+        "metric": "batched_scan_throughput", "value": n * args.steps / GIB / dev_s, "unit": "GiB/s",
+        "steps": args.steps, "warmup": args.warmup, "ms_per_step": dev_s / args.steps * 1e3,
+        "workload": "cfg2's automaton and haystack cut into documents of log-uniform length in [16 B, 16 KiB], "
+                    "find_overlapping_iter of every document in one batch call",
+        "haystack_bytes": n, "documents": int(offs.size - 1), "mean_document_bytes": n / (offs.size - 1),
+        "engine": {2: "prefilter_kernel", 3: "seq_docs_kernel"}.get(engine, engine),
+        "matches": len(got), "scan_ms": sum(scan_ms) / len(scan_ms), "order_ms": sum(order_ms) / len(order_ms),
+        "timing": "CUDA events inside the library: scan + order of the batch call on the search stream",
+        "wall_ms_per_step": wall / args.steps * 1e3,
+        "check": {"single_span_matches": len(single), "straddling_dropped": int((~keep).sum()),
+                  "count": len(mine), "fnv": f"{fnv:016x}", "equal": True},
+        "call_overhead": {"documents": k, "matches": batch_n, "one_call_per_document_ms": per_doc_s * 1e3,
+                          "one_batch_call_ms": batch_s * 1e3,
+                          "timing": "host clock around calls that end in a device synchronise"},
+        "clocks": clocks.summary()}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
