@@ -153,6 +153,7 @@ def _declare(lib):
     lib.acg_find_iter_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _vp, _u64, C.POINTER(_u64)]
     lib.acg_find_overlapping_batch.argtypes = lib.acg_find_iter_batch.argtypes
     lib.acg_is_match_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _vp]
+    lib.acg_find_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _i, _vp, _vp]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -707,6 +708,25 @@ class AhoCorasick:
         if rc:
             self._raise(rc)
         return flags[: offs.size - 1].astype(bool)
+
+    def find_batch_np(self, docs, anchored=Anchored.No, earliest=False):
+        """try_find of every document: (found, bool [n_docs]; records, DOC_MATCH_DTYPE [n_docs]).  A document
+        without a match has found False and the record (pid 0, doc, 0, 0)."""
+        keep, ptr, n, on_dev, offs = _batch_input(docs)
+        n_docs = offs.size - 1
+        found = np.empty(max(n_docs, 1), dtype=np.uint8)
+        out = np.empty(max(n_docs, 1), DOC_MATCH_DTYPE)
+        rc = _lib.acg_find_batch(self._h, ptr, on_dev, n, offs.ctypes.data, n_docs, int(anchored), int(earliest),
+                                 out.ctypes.data, found.ctypes.data)
+        if rc:
+            self._raise(rc)
+        return found[:n_docs].astype(bool), out[:n_docs]
+
+    def find_batch(self, docs, anchored=Anchored.No, earliest=False):
+        """try_find of every document: one Match, or None, per document."""
+        found, r = self.find_batch_np(docs, anchored, earliest)
+        return [Match(p, s, e) if f else None
+                for f, p, s, e in zip(found.tolist(), r["pid"].tolist(), r["start"].tolist(), r["end"].tolist())]
 
     # ---- replace / stream: host-side glue over find_iter, as in the reference -------------------
     @staticmethod

@@ -1752,13 +1752,16 @@ int find_iter_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uin
   return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, mode);
 }
 
-enum BatchKind { kBatchFindIter = 0, kBatchOverlapping = 1, kBatchIsMatch = 2 };
+enum BatchKind { kBatchFindIter = 0, kBatchOverlapping = 1, kBatchIsMatch = 2, kBatchFind = 3 };
 
-// acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch (include/acb200.h).
+// acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch / acg_find_batch (include/acb200.h).
+// is_match and find give one result per document: flags[n_docs] (find: found) and, for find, out[n_docs].
 int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                const uint64_t* offs, uint64_t n_docs, int anchored, acg_match* out, uint64_t cap, uint64_t* n_out,
-               uint8_t* flags) {
-  if (!a || !offs || (what == kBatchIsMatch ? (!flags && n_docs) : !n_out)) return ACG_E_INVALID_ARG;
+               uint8_t* flags, int earliest = 0) {
+  const bool per_doc = what == kBatchIsMatch || what == kBatchFind;
+  if (!a || !offs || (per_doc ? n_docs && (!flags || (what == kBatchFind && !out)) : !n_out))
+    return ACG_E_INVALID_ARG;
   if (n_out) *n_out = 0;
   if (n_docs >= (1ull << 32)) return ACG_E_INVALID_ARG;
   for (uint64_t i = 0; i < n_docs; ++i)
@@ -1773,9 +1776,15 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if ((rc = check_start(a->h, anchored))) return rc;
   if (!a->on_device) return ACG_E_NO_DEVICE;
   if (n_docs == 0) return ACG_OK;
+  const bool leftmost = a->h.match_kind != ACG_STANDARD;
+  // find: acg_find's packed-prefilter rule (an unanchored leftmost try_find returns the prefilter's confirmed
+  // leftmost match, src/automaton.rs:1304-1309) and its engine rule (`earliest` on a leftmost automaton
+  // reports the first match state entered, which the per-start scan does not model)
+  if (earliest && !anchored && leftmost && a->h.prefilter_kind == ACG_PRE_PACKED) earliest = 0;
+  const bool pf_ok = a->pf.supported && !anchored && !(earliest && leftmost);
   const int engine = a->engine_override;
-  if (engine == ACG_ENGINE_PREFILTER && (!a->pf.supported || anchored)) return ACG_E_INVALID_ARG;
-  const bool use_pf = engine != ACG_ENGINE_SEQUENTIAL && a->pf.supported && !anchored;
+  if (engine == ACG_ENGINE_PREFILTER && !pf_ok) return ACG_E_INVALID_ARG;
+  const bool use_pf = engine != ACG_ENGINE_SEQUENTIAL && pf_ok;
   DeviceGuard guard(a->device);
   WsLease lease(a);
   if (lease.rc) return lease.rc;
@@ -1783,6 +1792,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   w.stats.engine = use_pf ? ACG_ENGINE_PREFILTER : ACG_ENGINE_SEQUENTIAL;
   const uint64_t span_start = offs[0], span_end = offs[n_docs], nd1 = n_docs + 1;
   if ((rc = ensure_docs(w, nd1))) return rc;
+  if (what == kBatchFind && (rc = ensure_seq(w, n_docs))) return rc;  // the records, at index doc
   uint64_t* d_offs = w.d_docs;
   unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(w.d_docs + w.docs_cap);
   unsigned long long* d_incl = d_counts + w.docs_cap;
@@ -1794,8 +1804,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     if ((rc = stage_host_span(a, hay, span_start, span_end, &d_base, pipelined))) return rc;
     readable = span_end + 32;
   }
-  auto fetch_flags = [&]() -> int {
+  auto fetch_per_doc = [&]() -> int {
     CK(cudaMemcpyAsync(flags, w.d_doc_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
+    if (what == kBatchFind) CK(cudaMemcpyAsync(out, w.d_seq, n_docs * 24, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaStreamSynchronize(w.stream));
     return ACG_OK;
   };
@@ -1809,13 +1820,19 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     p.anchored = anchored;
     p.match_kind = a->h.match_kind;
     p.overlapping = what == kBatchOverlapping;
-    p.single = what == kBatchIsMatch;
+    p.single = per_doc;
+    p.earliest = what == kBatchIsMatch || earliest;
     CK(cudaEventRecord(w.ev0, w.stream));
-    if (what == kBatchIsMatch) {
+    if (per_doc) {
       p.flags = w.d_doc_flags;
+      if (what == kBatchFind) {
+        p.find = 1;
+        p.out = w.d_seq;
+        p.cap = n_docs;
+      }
       CK(acb::launch_seq_docs(a->dev, p, w.stream));
       CK(cudaEventRecord(w.ev1, w.stream));
-      if ((rc = fetch_flags())) return rc;
+      if ((rc = fetch_per_doc())) return rc;
       cudaEventElapsedTime(&ms, w.ev0, w.ev1);
       w.stats.scan_ms = ms;
       w.stats.launches += 1;
@@ -1863,12 +1880,15 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   DocBatch docs;
   docs.d_offsets = d_offs;
   docs.n = n_docs;
-  docs.unordered = what == kBatchIsMatch;
+  docs.unordered = per_doc;
   TupleResult r;
   if ((rc = run_prefilter(a, d_base, readable, span_start, span_end, pf_mode, &r, pipelined ? hay : nullptr,
                           UINT64_MAX, UINT64_MAX, &docs)))
     return rc;
-  if (what == kBatchIsMatch) {
+  if (per_doc) {
+    // is_match: the documents of the tuples.  find: per document, the tuple with the smallest key (mode 1: the
+    // best match at the smallest start; mode 2: the smallest end, longest first, then list order -- entry 0 of
+    // the first match state entered), the first tuple acg_find takes from the same keys in sorted order.
     acb::DocFlagsLaunch f;
     f.keys = w.d_keys[r.sorted_buf];
     f.pids = w.d_pids[r.sorted_buf];
@@ -1880,13 +1900,20 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     f.n_docs = n_docs;
     f.flags = w.d_doc_flags;
     CK(cudaEventRecord(w.ev2, w.stream));
-    CK(cudaMemsetAsync(w.d_doc_flags, 0, n_docs, w.stream));
-    CK(acb::launch_doc_flags(f, w.stream));
+    if (what == kBatchFind) {
+      f.best = d_counts;
+      f.out = w.d_seq;
+      CK(acb::launch_doc_first(f, w.stream));
+      w.stats.launches += 3;
+    } else {
+      CK(cudaMemsetAsync(w.d_doc_flags, 0, n_docs, w.stream));
+      CK(acb::launch_doc_flags(f, w.stream));
+      w.stats.launches += 1;
+    }
     CK(cudaEventRecord(w.ev3, w.stream));
-    if ((rc = fetch_flags())) return rc;
+    if ((rc = fetch_per_doc())) return rc;
     cudaEventElapsedTime(&ms, w.ev2, w.ev3);
     w.stats.order_ms = ms;
-    w.stats.launches += 1;
     return ACG_OK;
   }
   if (what == kBatchFindIter && (rc = run_chain(a, chain_mode, &r))) return rc;
@@ -2243,6 +2270,12 @@ int acg_is_match_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, 
                        const uint64_t* doc_offsets, uint64_t n_docs, int anchored, uint8_t* flags) {
   return batch_impl(a, kBatchIsMatch, hay, hay_on_device != 0, hay_len, doc_offsets, n_docs, anchored, nullptr, 0,
                     nullptr, flags);
+}
+int acg_find_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                   const uint64_t* doc_offsets, uint64_t n_docs, int anchored, int earliest, acg_doc_match* out,
+                   uint8_t* found) {
+  return batch_impl(a, kBatchFind, hay, hay_on_device != 0, hay_len, doc_offsets, n_docs, anchored,
+                    reinterpret_cast<acg_match*>(out), n_docs, nullptr, found, earliest != 0);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

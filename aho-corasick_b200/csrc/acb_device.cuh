@@ -93,7 +93,8 @@ cudaError_t launch_seq_find(const DfaDev& dfa, const SeqLaunch& p, cudaStream_t 
 // prefilter engine does not apply).  Two launches: the count pass (incl == nullptr) fills
 // counts[n_docs] -- or flags[n_docs] for is_match -- and after an inclusive scan of the counts the fill
 // pass writes each document's records at out[incl[doc - 1] * 3] as (pid | doc << 32, start, end) with
-// offsets relative to the document, the acg_doc_match layout.  A long document is one thread's walk.
+// offsets relative to the document, the acg_doc_match layout.  find: one launch (`find`).  A long
+// document is one thread's walk.
 struct SeqDocsLaunch {
   const uint8_t* hay;
   const uint64_t* doc_offsets;  // [n_docs + 1], haystack offsets
@@ -101,9 +102,12 @@ struct SeqDocsLaunch {
   int anchored;
   int match_kind;
   int overlapping;              // 1: find_overlapping_iter, 0: find_iter
-  int single;                   // 1: stop at the first match (is_match)
+  int single;                   // 1: stop at the first match (is_match, find)
+  int earliest;                 // find_iter, find: as acg_find's `earliest` (forced on for Standard)
+  int find;                     // find (with single): one pass, the first match or (0 | doc << 32, 0, 0) at
+                                // out[doc * 3] and flags[doc] = found
   unsigned long long* counts;   // count pass: [n_docs]
-  uint8_t* flags;               // count pass, is_match: [n_docs] instead of counts
+  uint8_t* flags;               // count pass, is_match / find: [n_docs] instead of counts
   const unsigned long long* incl;   // fill pass: [n_docs] inclusive scan of counts
   uint64_t* out;
   uint64_t cap;                 // records
@@ -113,6 +117,9 @@ cudaError_t inclusive_sum_u64(void* d_temp, size_t& temp_bytes, const unsigned l
                               uint64_t n, cudaStream_t s);
 
 // is_match over a batch on the prefilter engine: flags[doc] = 1 for the document of each of n tuples.
+// find over a batch (best != nullptr): the tuple with the smallest key of each document -- its first match,
+// since the keys of one document order its candidates as try_find prefers them -- written at out[doc * 3] in
+// the acg_doc_match layout, flags[doc] = found; (0 | doc << 32, 0, 0) and 0 for a document without one.
 struct DocFlagsLaunch {
   const uint64_t* keys;
   const uint32_t* pids;
@@ -123,8 +130,12 @@ struct DocFlagsLaunch {
   const uint64_t* doc_offsets;  // [n_docs + 1]
   uint64_t n_docs;
   uint8_t* flags;
+  unsigned long long* best = nullptr;  // find: [n_docs] scratch, the smallest key per document
+  uint64_t* out = nullptr;             // find: [n_docs * 3]
 };
 cudaError_t launch_doc_flags(const DocFlagsLaunch& f, cudaStream_t s);
+// find: three launches (clear, per-document minimum key, write the minimum's record)
+cudaError_t launch_doc_first(const DocFlagsLaunch& f, cudaStream_t s);
 
 // K3/K3b: position-parallel k-gram prefilter fused with the anchored DFA verify.
 // Plays the role of the reference's packed/Teddy prefilter (src/packed/teddy/

@@ -7,6 +7,8 @@
 //   Kseq seq_find_kernel          single-lane FindIter/try_find (anchored inputs,
 //                                 empty-pattern automata)
 //        seq_docs_kernel          the same per document of a batch, one thread each
+//        doc_flags_kernel         per-document is_match / first match of a batch's
+//        doc_first_kernel         prefilter tuples
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
 #ifndef ACB_PTX_HEADER
@@ -262,7 +264,8 @@ struct SumOp {
 // One thread per document of a batch.  Count pass (incl == nullptr): counts[doc] = its number of
 // matches, or flags[doc] = (a match exists) when flags is given.  Fill pass: the document's records from
 // index incl[doc - 1] (the matches of the documents before it) on, tagged with the document
-// (doc << 32 in the pid word, offsets relative to the document's first byte).
+// (doc << 32 in the pid word, offsets relative to the document's first byte).  find: the count pass with
+// flags, the document's one record written at index doc.
 constexpr int kSeqDocThreads = 128;
 template <bool OVERLAPPING>
 __global__ void __launch_bounds__(kSeqDocThreads) seq_docs_kernel(DfaDev d, SeqDocsLaunch p) {
@@ -270,14 +273,19 @@ __global__ void __launch_bounds__(kSeqDocThreads) seq_docs_kernel(DfaDev d, SeqD
   if (doc >= p.n_docs) return;
   const uint64_t lo = p.doc_offsets[doc], hi = p.doc_offsets[doc + 1];
   const bool fill = p.incl != nullptr;
-  uint64_t* out = fill ? p.out : nullptr;
-  const unsigned long long first = fill && doc ? p.incl[doc - 1] : 0;
+  uint64_t* out = fill || p.find ? p.out : nullptr;
+  const unsigned long long first = p.find ? doc : (fill && doc ? p.incl[doc - 1] : 0);
   const uint64_t tag = doc << 32;
+  if (p.find) {  // the record of "no match", overwritten by the match if there is one
+    out[doc * 3 + 0] = tag;
+    out[doc * 3 + 1] = 0;
+    out[doc * 3 + 2] = 0;
+  }
   unsigned long long n;
   if constexpr (OVERLAPPING) {
     n = seq_overlapping(d, p.hay, lo, hi, out, first, p.cap, tag);
   } else {
-    const bool earliest = p.match_kind == 0 || p.single != 0;
+    const bool earliest = p.match_kind == 0 || p.earliest != 0;
     n = seq_find_iter(d, p.hay, lo, hi, p.anchored != 0, earliest, p.single != 0, out, first, p.cap, tag, lo);
   }
   if (fill) return;
@@ -285,19 +293,72 @@ __global__ void __launch_bounds__(kSeqDocThreads) seq_docs_kernel(DfaDev d, SeqD
   else p.counts[doc] = n;
 }
 
-// is_match over a batch, prefilter engine: flags[doc] = 1 for the document of every tuple (key as
-// ChainLaunch::mode: 1 = start_rel << 24 | len, 0 = end_rel << 24 | tie).
+#ifdef ACB_EMULATE
+// The dry-run runtime (tests/emu) has no atomicMin; it runs one thread at a time between synchronisation
+// points, so a plain read-modify-write is atomic there.
+inline unsigned long long atomicMin(unsigned long long* p, unsigned long long v) {
+  const unsigned long long o = *p;
+  if (v < o) *p = v;
+  return o;
+}
+#endif
+
+// The document that holds haystack offset s, which lies in [doc_offsets[0], doc_offsets[n_docs]): the
+// last one that starts at or before s, found by an upper-bound search for the first document end past s.
+// (An empty document's end is its start, so the search never stops at one.)
+__device__ __forceinline__ uint64_t doc_of(const uint64_t* offs, uint64_t n_docs, uint64_t s) {
+  uint64_t lo = 1, hi = n_docs;
+  while (lo < hi) {
+    const uint64_t mid = lo + ((hi - lo) >> 1);
+    if (offs[mid] > s) hi = mid; else lo = mid + 1;
+  }
+  return lo - 1;
+}
+
+// The haystack start offset of tuple i (key as ChainLaunch::mode: 1 = start_rel << 24 | len,
+// 0 = end_rel << 24 | tie).
+__device__ __forceinline__ uint64_t tuple_start(const DocFlagsLaunch& f, uint64_t i) {
+  const uint64_t key = f.keys[i];
+  return f.span_start + (f.mode == 1 ? key >> kTieBits : (key >> kTieBits) - f.pattern_lens[f.pids[i]]);
+}
+
+// Over the n tuples of a prefilter scan.  is_match: flags[doc] = 1 for the document of every tuple.
+// find (best != nullptr): best[doc] = the smallest key of the document's tuples.
 __global__ void doc_flags_kernel(DocFlagsLaunch f) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= f.n) return;
+  const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, tuple_start(f, i));
+  if (f.best) atomicMin(f.best + doc, (unsigned long long)f.keys[i]);
+  else f.flags[doc] = 1;
+}
+
+// find: clear best[] and flags[], and give every document the record of "no match".
+__global__ void doc_first_clear_kernel(DocFlagsLaunch f) {
+  const uint64_t doc = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (doc >= f.n_docs) return;
+  f.best[doc] = ~0ull;
+  f.flags[doc] = 0;
+  f.out[doc * 3 + 0] = doc << 32;
+  f.out[doc * 3 + 1] = 0;
+  f.out[doc * 3 + 2] = 0;
+}
+
+// find, after doc_flags_kernel: the tuple holding its document's smallest key writes the document's record
+// (decoded as acg_find decodes its first tuple, offsets relative to the document).  Keys are unique within
+// a document, so one tuple per document writes.
+__global__ void doc_first_kernel(DocFlagsLaunch f) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= f.n) return;
+  const uint64_t s = tuple_start(f, i);
+  const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, s);
   const uint64_t key = f.keys[i];
-  const uint64_t s = f.span_start + (f.mode == 1 ? key >> kTieBits : (key >> kTieBits) - f.pattern_lens[f.pids[i]]);
-  uint64_t lo = 1, hi = f.n_docs;  // the first document end past s
-  while (lo < hi) {
-    const uint64_t mid = lo + ((hi - lo) >> 1);
-    if (f.doc_offsets[mid] > s) hi = mid; else lo = mid + 1;
-  }
-  f.flags[lo - 1] = 1;
+  if (key != f.best[doc]) return;
+  const uint32_t pid = f.pids[i];
+  const uint64_t base = f.doc_offsets[doc];
+  f.out[doc * 3 + 0] = (uint64_t)pid | doc << 32;
+  f.out[doc * 3 + 1] = s - base;
+  f.out[doc * 3 + 2] = s + (f.mode == 1 ? key & kTieMask : f.pattern_lens[pid]) - base;
+  f.flags[doc] = 1;
 }
 
 // Records built in shared memory and stored as 16-byte vectors: the target may be another GPU's HBM
@@ -400,6 +461,15 @@ cudaError_t launch_seq_docs(const DfaDev& dfa, const SeqDocsLaunch& p, cudaStrea
 cudaError_t launch_doc_flags(const DocFlagsLaunch& f, cudaStream_t s) {
   if (f.n == 0) return cudaSuccess;
   ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_doc_first(const DocFlagsLaunch& f, cudaStream_t s) {
+  if (f.n_docs == 0) return cudaSuccess;
+  ACB_LAUNCH(doc_first_clear_kernel, (unsigned)((f.n_docs + 255) / 256), 256, 0, s, f);
+  if (f.n == 0) return cudaGetLastError();
+  ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
+  ACB_LAUNCH(doc_first_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
   return cudaGetLastError();
 }
 

@@ -220,6 +220,16 @@ int acg_find_overlapping_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_o
 /* AhoCorasick::is_match(doc) for every document: flags[d] = 0 / 1 */
 int acg_is_match_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
                        const uint64_t* doc_offsets, uint64_t n_docs, int anchored, uint8_t* flags);
+/* AhoCorasick::try_find(Input::new(doc).anchored(a).earliest(e)) for every document.
+ * found[d] = 1 and out[d] = {pid, d, start, end} (offsets relative to the document) when the
+ * single-haystack acg_find on document d alone, span (0, len), reports a match; otherwise
+ * found[d] = 0 and out[d] = {0, d, 0, 0}.  Both arrays have n_docs entries in host memory.
+ * One output slot per document: no overflow protocol.  `earliest` follows acg_find, including its
+ * packed-prefilter rule; an ACG_ENGINE_PREFILTER override the input cannot use (anchored, no
+ * prefilter plan, `earliest` on a leftmost automaton) gives ACG_E_INVALID_ARG. */
+int acg_find_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                   const uint64_t* doc_offsets, uint64_t n_docs, int anchored, int earliest,
+                   acg_doc_match* out, uint8_t* found);
 
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END

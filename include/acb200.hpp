@@ -329,6 +329,28 @@ class AhoCorasick {
                                    Anchored a = Anchored::No) const {
     return std::move(try_is_match_batch(haystack, offsets, a).unwrap());
   }
+  // try_find of every document (acg_find_batch): its first match, or nullopt
+  using FirstPerDoc = std::vector<std::optional<Match>>;
+  Result<FirstPerDoc> try_find_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                     Anchored a = Anchored::No, bool earliest = false) const {
+    Result<FirstPerDoc> r;
+    if (offsets.empty()) { r.error = ACG_E_INVALID_ARG; return r; }
+    const uint64_t n_docs = offsets.size() - 1;
+    std::vector<acg_doc_match> out(n_docs);
+    std::vector<uint8_t> found(n_docs);
+    r.error = acg_find_batch(h_, reinterpret_cast<const uint8_t*>(haystack.data()), 0, haystack.size(), offsets.data(),
+                             n_docs, int(a), int(earliest), out.data(), found.data());
+    if (r.error == 0) {
+      r.value.resize(n_docs);
+      for (uint64_t d = 0; d < n_docs; ++d)
+        if (found[d]) r.value[d] = Match(out[d].pid, out[d].start, out[d].end);
+    }
+    return r;
+  }
+  FirstPerDoc find_batch(std::string_view haystack, const std::vector<uint64_t>& offsets, Anchored a = Anchored::No,
+                         bool earliest = false) const {
+    return std::move(try_find_batch(haystack, offsets, a, earliest).unwrap());
+  }
 
   // replace_all_with / replace_all_with_bytes, :834 / :887 (src/automaton.rs:498-550)
   template <class F>

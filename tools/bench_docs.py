@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
-"""Batched search over many documents in one device call (acg_find_overlapping_batch).
+"""Batched search over many documents in one device call (acg_find_overlapping_batch, acg_find_batch).
 
     python tools/bench_docs.py [--hay-gib 4] [--steps 20] [--warmup 5] [--engine 0]
+                               [--call overlapping|find] [--workload cfg2|cfg3]
 
 cfg 2's automaton and haystack (same seeds as bench.py), device-resident, cut at seeded boundaries into
 documents of log-uniform length in [16 B, 16 KiB] (~1.8 M documents, mean ~2.4 KiB at 4 GiB).  Prints one
@@ -11,6 +12,11 @@ card's name and power limit, and two checks outside the timed region:
     straddle a document boundary, record for record (count and FNV-1a reported);
   * call overhead on the first 10 000 documents: one single-haystack call per document against one batch
     call over the same documents (same match count).
+
+--call find times find_batch (the first match of every document: scan + per-document reduction), on cfg 2
+or on cfg 3 (leftmost-first, case-insensitive, built as bench.py builds it: the leftmost reduction).  Its
+checks: find_batch equals the first find_iter_batch record of every document, and 10 000 single find
+calls against one find_batch call over the same documents (host haystack, same results).
 """
 import argparse
 import importlib.util
@@ -45,13 +51,80 @@ def fnv1a(rec):
     return h
 
 
+def bench_find(args, ac, d_hay, offs, ClockSampler):
+    """--call find: find_batch over the whole batch, timed; then its checks."""
+    import numpy as np
+    import aho_corasick_b200 as ab
+    n, n_docs = d_hay.numel(), offs.size - 1
+    batch = (d_hay, offs)
+    for _ in range(args.warmup):
+        found, rec = ac.find_batch_np(batch)
+    kernel_ms, scan_ms, order_ms = [], [], []
+    with ClockSampler(0) as clocks:
+        t0 = time.perf_counter()
+        for _ in range(args.steps):
+            found, rec = ac.find_batch_np(batch)
+            st = ac.last_stats()
+            kernel_ms.append(st["scan_ms"] + st["order_ms"])
+            scan_ms.append(st["scan_ms"])
+            order_ms.append(st["order_ms"])
+        wall = time.perf_counter() - t0
+    engine, tuples = int(st["engine"]), int(st["raw_matches"])
+    # check 1: the first find_iter_batch record of every document
+    it = ac.find_iter_batch_np(batch)
+    idx = np.flatnonzero(np.r_[True, it["doc"][1:] != it["doc"][:-1]]) if len(it) else np.zeros(0, np.int64)
+    first_docs = it["doc"][idx].astype(np.int64)
+    want = np.zeros(n_docs, ab.DOC_MATCH_DTYPE)
+    want["doc"] = np.arange(n_docs)
+    want[first_docs] = it[idx]
+    assert np.array_equal(np.flatnonzero(found), first_docs), "found flags differ from find_iter_batch"
+    assert rec.tobytes() == want.tobytes(), "records differ from find_iter_batch's first records"
+    # check 2: call overhead on the first 10 000 documents, host haystack for both sides
+    k = min(10_000, n_docs)
+    sub = offs[: k + 1]
+    head = d_hay[: int(sub[-1])].cpu().numpy()
+    docs = [head[int(sub[d]):int(sub[d + 1])] for d in range(k)]
+    for d in range(min(k, 100)):  # warm
+        ac.find(docs[d])
+    t0 = time.perf_counter()
+    single = [ac.find(doc) for doc in docs]
+    per_doc_s = time.perf_counter() - t0
+    ac.find_batch((head, sub))
+    t0 = time.perf_counter()
+    batched = ac.find_batch((head, sub))
+    batch_s = time.perf_counter() - t0
+    assert [m and m.as_tuple() for m in single] == [m and m.as_tuple() for m in batched]
+    dev_s = sum(kernel_ms) / 1e3
+    kind = "cfg3's automaton (leftmost-first, case-insensitive)" if args.workload == "cfg3" else "cfg2's automaton"
+    print(json.dumps({
+        "metric": "batched_find_throughput", "value": n * args.steps / GIB / dev_s, "unit": "GiB/s",
+        "steps": args.steps, "warmup": args.warmup, "ms_per_step": dev_s / args.steps * 1e3,
+        "workload": f"{kind} and {args.workload}'s haystack cut into documents of log-uniform length in "
+                    "[16 B, 16 KiB], the first match of every document (find) in one batch call",
+        "haystack_bytes": n, "documents": n_docs, "mean_document_bytes": n / n_docs,
+        "engine": {2: "prefilter_kernel + doc_first_kernel", 3: "seq_docs_kernel"}.get(engine, engine),
+        "documents_with_a_match": int(found.sum()), "tuples_reduced": tuples,
+        "scan_ms": sum(scan_ms) / len(scan_ms), "order_ms": sum(order_ms) / len(order_ms),
+        "timing": "CUDA events inside the library: scan + per-document reduction of the batch call",
+        "wall_ms_per_step": wall / args.steps * 1e3,
+        "check": {"first_find_iter_record_per_document": True, "find_iter_matches": len(it)},
+        "call_overhead": {"documents": k, "documents_with_a_match": sum(m is not None for m in batched),
+                          "one_call_per_document_ms": per_doc_s * 1e3, "one_batch_call_ms": batch_s * 1e3,
+                          "timing": "host clock around calls that end in a device synchronise, host haystack"},
+        "clocks": clocks.summary()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--hay-gib", type=float, default=4.0)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--engine", type=int, default=0, help="0 auto, 3 the per-document sequential kernel")
+    ap.add_argument("--call", default="overlapping", choices=["overlapping", "find"])
+    ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg3"])
     args = ap.parse_args()
+    if args.call == "overlapping" and args.workload != "cfg2":
+        ap.error("find_overlapping_iter needs cfg 2's Standard automaton")
     import numpy as np
     import torch
     import aho_corasick_b200 as ab
@@ -60,12 +133,17 @@ def main():
     ClockSampler = clock_sampler()
     n = int(args.hay_gib * GIB)
     n -= n % 4096
-    pats = W.config_patterns("cfg2")
-    ac = ab.AhoCorasick.builder().kind(ab.AhoCorasickKind.DFA).build(pats).set_engine(args.engine)
+    pats = W.config_patterns(args.workload)
+    b = ab.AhoCorasick.builder().kind(ab.AhoCorasickKind.DFA)
+    if args.workload == "cfg3":
+        b.ascii_case_insensitive(True).match_kind(ab.MatchKind.LeftmostFirst)
+    ac = b.build(pats).set_engine(args.engine)
     d_hay = torch.empty(n, dtype=torch.uint8, device="cuda")
-    W.torch_fill_config("cfg2", d_hay, pats)
+    W.torch_fill_config(args.workload, d_hay, pats)
     torch.cuda.synchronize()
     offs = W.doc_offsets(n, 0xD0C5)
+    if args.call == "find":
+        return bench_find(args, ac, d_hay, offs, ClockSampler)
     batch = (d_hay, offs)
     for _ in range(args.warmup):
         got = ac.find_overlapping_iter_batch_np(batch)
