@@ -49,7 +49,7 @@ struct Workspace {
   uint32_t* d_pids[2] = {nullptr, nullptr};
   unsigned long long* d_counter = nullptr;
   unsigned long long* h_counter = nullptr;  // pinned
-  void* d_temp = nullptr;
+  void* d_temp = nullptr;  // CUB temporary storage (cub_call): a search's CUB calls run in order on `stream`
   size_t temp_bytes = 0;
   uint64_t* h_keys = nullptr;  // pinned staging
   uint32_t* h_pids = nullptr;
@@ -58,8 +58,6 @@ struct Workspace {
   uint64_t d_hay_cap = 0;
   uint64_t* d_scratch = nullptr;  // chain resolution: end offsets / prefix max [cap]
   uint8_t* d_flags = nullptr;     // [cap]
-  void* d_temp2 = nullptr;        // scan / select temp
-  size_t temp2_bytes = 0;
   uint64_t chain_cap = 0;
   uint64_t* d_seq = nullptr;  // sequential engine output [cap*3]
   uint64_t seq_cap = 0;
@@ -74,8 +72,6 @@ struct Workspace {
   uint64_t* d_docs = nullptr;
   uint8_t* d_doc_flags = nullptr;
   uint64_t docs_cap = 0;
-  void* d_temp3 = nullptr;  // scan temp
-  size_t temp3_bytes = 0;
 };
 
 }  // namespace
@@ -162,8 +158,8 @@ void destroy_workspace(Workspace& w) {
   if (w.stream) cudaStreamSynchronize(w.stream);
   for (int i = 0; i < 2; ++i) { cudaFree(w.d_keys[i]); cudaFree(w.d_pids[i]); }
   cudaFree(w.d_counter); cudaFree(w.d_temp); cudaFree(w.d_hay); cudaFree(w.d_seq);
-  cudaFree(w.d_scratch); cudaFree(w.d_flags); cudaFree(w.d_temp2);
-  cudaFree(w.d_docs); cudaFree(w.d_doc_flags); cudaFree(w.d_temp3);
+  cudaFree(w.d_scratch); cudaFree(w.d_flags);
+  cudaFree(w.d_docs); cudaFree(w.d_doc_flags);
   if (w.h_counter) cudaFreeHost(w.h_counter);
   if (w.h_keys) cudaFreeHost(w.h_keys);
   if (w.h_pids) cudaFreeHost(w.h_pids);
@@ -726,17 +722,30 @@ int ensure_tuple_cap(Workspace& w, uint64_t cap) {
     w.d_keys[i] = nullptr;
     w.d_pids[i] = nullptr;
   }
-  if (w.d_temp) { cudaFree(w.d_temp); w.d_temp = nullptr; }
   w.cap = 0;
   for (int i = 0; i < 2; ++i) {
     CK(cudaMalloc(&w.d_keys[i], cap * 8));
     CK(cudaMalloc(&w.d_pids[i], cap * 4));
   }
-  size_t tb = 0;
-  CK(acb::sort_pairs(nullptr, tb, w.d_keys[0], w.d_keys[1], w.d_pids[0], w.d_pids[1], cap, 64, w.stream));
-  CK(cudaMalloc(&w.d_temp, std::max<size_t>(tb, 16)));
-  w.temp_bytes = tb;
   w.cap = cap;
+  return ACG_OK;
+}
+
+// One CUB call `f(d_temp, temp_bytes)` on the workspace's temporary storage: sized by a query
+// (d_temp == nullptr, which CUB answers without doing the work) and grown if the call needs more.
+template <class F>
+int cub_call(Workspace& w, F f) {
+  size_t tb = 0;
+  CK(f(nullptr, tb));
+  if (!w.d_temp || tb > w.temp_bytes) {
+    cudaFree(w.d_temp);
+    w.d_temp = nullptr;
+    w.temp_bytes = 0;
+    CK(cudaMalloc(&w.d_temp, std::max<size_t>(tb, 16)));
+    w.temp_bytes = std::max<size_t>(tb, 16);
+  }
+  tb = w.temp_bytes;
+  CK(f(w.d_temp, tb));
   return ACG_OK;
 }
 
@@ -823,72 +832,6 @@ struct DocBatch {
   uint64_t n = 0;
   bool unordered = false;  // is_match: one list, no order step (only the documents of the tuples matter)
 };
-
-// K1 + K4 on a device-resident haystack; leaves `n` ordered tuples in
-// ws.d_keys[sorted_buf] / ws.d_pids[sorted_buf].
-int run_walk_overlapping(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uint64_t span_start,
-                         uint64_t span_end, TupleResult* res) {
-  Workspace& w = cur_ws();
-  const uint64_t n_bytes = span_end - span_start;
-  if (a->max_list_len >= (1u << acb::kTieBits)) return ACG_E_INVALID_ARG;
-  if (n_bytes >= (1ull << (64 - acb::kTieBits))) return ACG_E_INVALID_ARG;
-  int dev_sms = 132;
-  cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, a->device);
-  const uint64_t target_lanes = uint64_t(dev_sms) * 2048;
-  uint64_t seg_len = (n_bytes + target_lanes - 1) / std::max<uint64_t>(target_lanes, 1);
-  seg_len = std::max<uint64_t>(seg_len, 256);
-  seg_len = (seg_len + 15) & ~15ull;
-  // shard starts are placed so that (d_hay + span_start + k*seg_len) keeps the 16-byte
-  // phase of the first shard; the kernel handles the unaligned head per lane.
-  const uint64_t n_segs = std::max<uint64_t>((n_bytes + seg_len - 1) / seg_len, 1);
-  uint64_t cap = std::max<uint64_t>(w.cap, std::max<uint64_t>(1 << 20, n_bytes / 256));
-  for (int attempt = 0; attempt < 8; ++attempt) {
-    int rc = ensure_tuple_cap(w, cap);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
-    acb::WalkLaunch p;
-    p.hay = d_hay;
-    p.hay_len = readable;
-    p.span_start = span_start;
-    p.span_end = span_end;
-    p.seg_len = seg_len;
-    p.n_segs = n_segs;
-    p.keys = w.d_keys[0];
-    p.pids = w.d_pids[0];
-    p.counter = w.d_counter;
-    p.cap = w.cap;
-    CK(cudaEventRecord(w.ev0, w.stream));
-    CK(acb::launch_walk_overlapping(a->dev, p, w.stream));
-    CK(cudaEventRecord(w.ev1, w.stream));
-    CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream));
-    CK(cudaStreamSynchronize(w.stream));
-    cur_ws().stats.launches += 1;
-    const uint64_t want = *w.h_counter;
-    if (want > w.cap) { cap = want + want / 8 + 1024; continue; }  // overflow: grow and rescan
-    res->n = want;
-    cur_ws().stats.raw_matches = want;
-    float ms = 0;
-    cudaEventElapsedTime(&ms, w.ev0, w.ev1);
-    cur_ws().stats.scan_ms = ms;
-    if (want > 1) {
-      size_t tb = w.temp_bytes;
-      const int end_bit = std::min(64, acb::kTieBits + bits_for(n_bytes + 1));
-      CK(cudaEventRecord(w.ev2, w.stream));
-      CK(acb::sort_pairs(w.d_temp, tb, w.d_keys[0], w.d_keys[1], w.d_pids[0], w.d_pids[1], want, end_bit,
-                         w.stream));
-      CK(cudaEventRecord(w.ev3, w.stream));
-      CK(cudaStreamSynchronize(w.stream));
-      cudaEventElapsedTime(&ms, w.ev2, w.ev3);
-      cur_ws().stats.order_ms = ms;
-      cur_ws().stats.launches += 8;  // radix passes (upper bound, library code)
-      res->sorted_buf = 1;
-    } else {
-      res->sorted_buf = 0;
-    }
-    return ACG_OK;
-  }
-  return ACG_E_NOMEM;
-}
 
 // Bucketed emission of the prefilter engine (PrefilterLaunch::bucket_shift): the span's key offsets
 // [0, n_bytes] are cut into `n` ranges of 2^shift bytes, fixed before the first launch, and each
@@ -1010,13 +953,19 @@ int order_tuples(const acg_dfa* a, uint64_t want, uint64_t n_bytes, TupleResult*
   cur_ws().stats.raw_matches = want;
   res->sorted_buf = 0;
   if (want <= 1 && (bp.shift == 0 || want == 0)) return ACG_OK;  // (one bucketed tuple still has to move to slot 0)
-  size_t tb = w.temp_bytes;
   const int end_bit = std::min(64, acb::kTieBits + bits_for(n_bytes + 1));
   float ms = 0;
   CK(cudaEventRecord(w.ev2, w.stream));
+  // the list in buffer `from`, ordered into the other one
+  auto sort_list = [&](int from) {
+    return cub_call(w, [&](void* t, size_t& tb) {
+      return acb::sort_pairs(t, tb, w.d_keys[from], w.d_keys[1 - from], w.d_pids[from], w.d_pids[1 - from], want,
+                             end_bit, w.stream);
+    });
+  };
+  int rc;
   if (bp.shift == 0) {
-    CK(acb::sort_pairs(w.d_temp, tb, w.d_keys[0], w.d_keys[1], w.d_pids[0], w.d_pids[1], want, end_bit,
-                       w.stream));
+    if ((rc = sort_list(0))) return rc;
     cur_ws().stats.launches += 8;  // radix passes (library code, upper bound)
     res->sorted_buf = 1;
   } else {
@@ -1040,8 +989,7 @@ int order_tuples(const acg_dfa* a, uint64_t want, uint64_t n_bytes, TupleResult*
     } else {
       // a bucket overflowed: concatenate buckets and overflow list, radix sort of the whole list
       CK(acb::launch_compact_buckets(o, w.stream));
-      CK(acb::sort_pairs(w.d_temp, tb, w.d_keys[1], w.d_keys[0], w.d_pids[1], w.d_pids[0], want, end_bit,
-                         w.stream));
+      if ((rc = sort_list(1))) return rc;
       cur_ws().stats.launches += 9;
       res->sorted_buf = 0;
     }
@@ -1051,6 +999,55 @@ int order_tuples(const acg_dfa* a, uint64_t want, uint64_t n_bytes, TupleResult*
   cudaEventElapsedTime(&ms, w.ev2, w.ev3);
   cur_ws().stats.order_ms = ms;
   return ACG_OK;
+}
+
+// K1 + K4 on a device-resident haystack; leaves `n` ordered tuples in
+// ws.d_keys[sorted_buf] / ws.d_pids[sorted_buf].
+int run_walk_overlapping(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uint64_t span_start,
+                         uint64_t span_end, TupleResult* res) {
+  Workspace& w = cur_ws();
+  const uint64_t n_bytes = span_end - span_start;
+  if (a->max_list_len >= (1u << acb::kTieBits)) return ACG_E_INVALID_ARG;
+  if (n_bytes >= (1ull << (64 - acb::kTieBits))) return ACG_E_INVALID_ARG;
+  int dev_sms = 132;
+  cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, a->device);
+  const uint64_t target_lanes = uint64_t(dev_sms) * 2048;
+  uint64_t seg_len = (n_bytes + target_lanes - 1) / std::max<uint64_t>(target_lanes, 1);
+  seg_len = std::max<uint64_t>(seg_len, 256);
+  seg_len = (seg_len + 15) & ~15ull;
+  // shard starts are placed so that (d_hay + span_start + k*seg_len) keeps the 16-byte
+  // phase of the first shard; the kernel handles the unaligned head per lane.
+  const uint64_t n_segs = std::max<uint64_t>((n_bytes + seg_len - 1) / seg_len, 1);
+  uint64_t cap = std::max<uint64_t>(w.cap, std::max<uint64_t>(1 << 20, n_bytes / 256));
+  for (int attempt = 0; attempt < 8; ++attempt) {
+    int rc = ensure_tuple_cap(w, cap);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
+    acb::WalkLaunch p;
+    p.hay = d_hay;
+    p.hay_len = readable;
+    p.span_start = span_start;
+    p.span_end = span_end;
+    p.seg_len = seg_len;
+    p.n_segs = n_segs;
+    p.keys = w.d_keys[0];
+    p.pids = w.d_pids[0];
+    p.counter = w.d_counter;
+    p.cap = w.cap;
+    CK(cudaEventRecord(w.ev0, w.stream));
+    CK(acb::launch_walk_overlapping(a->dev, p, w.stream));
+    CK(cudaEventRecord(w.ev1, w.stream));
+    CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    cur_ws().stats.launches += 1;
+    const uint64_t want = *w.h_counter;
+    if (want > w.cap) { cap = want + want / 8 + 1024; continue; }  // overflow: grow and rescan
+    float ms = 0;
+    cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+    cur_ws().stats.scan_ms = ms;
+    return order_tuples(a, want, n_bytes, res, BucketPlan{}, 0);
+  }
+  return ACG_E_NOMEM;
 }
 
 // ---- pageable host haystacks ---------------------------------------------------------------------
@@ -1263,17 +1260,10 @@ int ensure_chain(Workspace& w, uint64_t n) {
   if (n <= w.chain_cap) return ACG_OK;
   if (w.d_scratch) cudaFree(w.d_scratch);
   if (w.d_flags) cudaFree(w.d_flags);
-  if (w.d_temp2) cudaFree(w.d_temp2);
-  w.d_scratch = nullptr; w.d_flags = nullptr; w.d_temp2 = nullptr; w.chain_cap = 0;
+  w.d_scratch = nullptr; w.d_flags = nullptr; w.chain_cap = 0;
   const uint64_t cap = std::max<uint64_t>(n, 1 << 16);
   CK(cudaMalloc(&w.d_scratch, cap * 8));
   CK(cudaMalloc(&w.d_flags, cap));
-  size_t t1 = 0, t2 = 0;
-  CK(acb::scan_max_u64(nullptr, t1, w.d_scratch, cap, w.stream));
-  CK(acb::select_flagged(nullptr, t2, w.d_keys[0], w.d_pids[0], w.d_flags, w.d_keys[1], w.d_pids[1],
-                         w.d_counter, cap, w.stream));
-  w.temp2_bytes = std::max(t1, t2);
-  CK(cudaMalloc(&w.d_temp2, std::max<size_t>(w.temp2_bytes, 16)));
   w.chain_cap = cap;
   return ACG_OK;
 }
@@ -1297,12 +1287,14 @@ int run_chain(const acg_dfa* a, int mode, TupleResult* r) {
   CK(cudaEventRecord(w.ev2, w.stream));
   CK(cudaMemsetAsync(w.d_flags, 0, r->n, w.stream));
   CK(acb::launch_chain_ends(c, w.stream));
-  size_t tb = w.temp2_bytes;
-  CK(acb::scan_max_u64(w.d_temp2, tb, w.d_scratch, r->n, w.stream));
+  if ((rc = cub_call(w, [&](void* t, size_t& tb) { return acb::scan_max_u64(t, tb, w.d_scratch, r->n, w.stream); })))
+    return rc;
   CK(acb::launch_chain_select(c, w.stream));
-  tb = w.temp2_bytes;
-  CK(acb::select_flagged(w.d_temp2, tb, w.d_keys[src], w.d_pids[src], w.d_flags, w.d_keys[dst],
-                         w.d_pids[dst], w.d_counter, r->n, w.stream));
+  if ((rc = cub_call(w, [&](void* t, size_t& tb) {
+         return acb::select_flagged(t, tb, w.d_keys[src], w.d_pids[src], w.d_flags, w.d_keys[dst], w.d_pids[dst],
+                                    w.d_counter, r->n, w.stream);
+       })))
+    return rc;
   CK(cudaEventRecord(w.ev3, w.stream));
   CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream));
   CK(cudaStreamSynchronize(w.stream));
@@ -1344,14 +1336,8 @@ int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, ac
   uint32_t doc = 0;
   for (uint64_t i = 0; i < r.n; ++i) {
     const uint32_t pid = w.h_pids[i];
-    uint64_t start, end;
-    if (key_mode == 1) {  // (start_rel << 24 | len)
-      start = span_start + (w.h_keys[i] >> acb::kTieBits);
-      end = start + (w.h_keys[i] & acb::kTieMask);
-    } else {              // (end_rel << 24 | tie)
-      end = span_start + (w.h_keys[i] >> acb::kTieBits);
-      start = end - plens[pid];
-    }
+    const acb::MatchSpan m = acb::decode_key(w.h_keys[i], pid, key_mode, span_start, plens);
+    uint64_t start = m.start, end = m.end;
     if (docs) {
       while (docs[doc + 1] <= start) ++doc;
       start -= docs[doc];
@@ -1370,26 +1356,31 @@ int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, ac
   return (out && r.n > cap) ? ACG_E_OVERFLOW : ACG_OK;
 }
 
+// The sequential engine over [span_start, span_end): the one-document form of seq_docs_kernel, which counts
+// and writes the records in the same walk.
 int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_t span_end,
             int anchored, int earliest, int single, acg_match* out, uint64_t cap, uint64_t* n_out) {
   Workspace& w = cur_ws();
   uint64_t scap = std::max<uint64_t>(std::max<uint64_t>(cap, 1024), w.seq_cap);
+  int rc = ensure_docs(w, 2);
+  if (rc) return rc;
+  const uint64_t bounds[2] = {span_start, span_end};
+  CK(cudaMemcpyAsync(w.d_docs, bounds, sizeof(bounds), cudaMemcpyHostToDevice, w.stream));
   for (int attempt = 0; attempt < 4; ++attempt) {
-    int rc = ensure_seq(w, scap);
-    if (rc) return rc;
-    acb::SeqLaunch p;
+    if ((rc = ensure_seq(w, scap))) return rc;
+    acb::SeqDocsLaunch p{};
     p.hay = d_hay;
-    p.span_start = span_start;
-    p.span_end = span_end;
+    p.doc_offsets = w.d_docs;
+    p.n_docs = 1;
     p.anchored = anchored;
     p.match_kind = a->h.match_kind;
     p.earliest = earliest;
     p.single = single;
+    p.counts = w.d_counter;
     p.out = w.d_seq;
-    p.counter = w.d_counter;
     p.cap = w.seq_cap;
     CK(cudaEventRecord(w.ev0, w.stream));
-    CK(acb::launch_seq_find(a->dev, p, w.stream));
+    CK(acb::launch_seq_docs(a->dev, p, w.stream));
     CK(cudaEventRecord(w.ev1, w.stream));
     CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaStreamSynchronize(w.stream));
@@ -1408,8 +1399,8 @@ int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_
       for (uint64_t i = 0; i < n; ++i) {
         out[i].pid = uint32_t(w.h_seq[i * 3]);
         out[i]._pad = 0;
-        out[i].start = w.h_seq[i * 3 + 1];
-        out[i].end = w.h_seq[i * 3 + 2];
+        out[i].start = span_start + w.h_seq[i * 3 + 1];
+        out[i].end = span_start + w.h_seq[i * 3 + 2];
       }
     }
     return ACG_OK;
@@ -1437,8 +1428,49 @@ int stage_host_span(const acg_dfa* a, const uint8_t* hay, uint64_t span_start, u
   float ms = 0;
   cudaEventElapsedTime(&ms, w.ev0, w.ev1);
   cur_ws().stats.h2d_ms = ms;
-  *d_base = w.d_hay + lead - span_start;  // never dereferenced outside [span_start, span_end)
   return ACG_OK;
+}
+
+// Where the kernels read the haystack: `base`, indexed with absolute offsets, and `readable` bytes behind it.
+// A host haystack is staged in the workspace; `pipelined` only allocates the room and leaves the copy from
+// `h_src` to run_prefilter, which overlaps it with the scan.
+struct Placement {
+  const uint8_t* base = nullptr;
+  uint64_t readable = 0;
+  const uint8_t* h_src = nullptr;
+};
+
+int place_input(const acg_dfa* a, const uint8_t* hay, bool on_device, uint64_t hay_len, uint64_t span_start,
+                uint64_t span_end, bool pipelined, Placement* p) {
+  if (on_device) {
+    p->base = hay;
+    p->readable = hay_len;
+    return ACG_OK;
+  }
+  p->readable = span_end + 32;  // the staging buffer has slack behind the span
+  if (pipelined) p->h_src = hay;
+  return stage_host_span(a, hay, span_start, span_end, &p->base, pipelined);
+}
+
+// acg_find / acg_find_batch: where the reference attaches its packed (Teddy) prefilter -- leftmost kinds
+// only -- an unanchored try_find returns what the prefilter reports, a confirmed leftmost match
+// (Candidate::Match, src/automaton.rs:1304-1309), whether or not `earliest` was asked for.
+int find_earliest(const acg_dfa* a, int anchored, int earliest) {
+  const bool packed = !anchored && a->h.match_kind != ACG_STANDARD && a->h.prefilter_kind == ACG_PRE_PACKED;
+  return earliest && !packed;
+}
+
+// The engine of a search, or ACG_E_INVALID_ARG.  The prefilter engine serves unanchored input of an
+// automaton with a plan, but not `earliest` on a leftmost automaton: that reports the first match STATE
+// entered (src/automaton.rs:1381-1383), which the per-start formulation does not model.  Otherwise the
+// call's `other` engine runs (the walk or the sequential engine), as does an override of it.  An
+// ACG_ENGINE_PREFILTER override the input cannot use is an error when `strict`, else `other` runs.
+int choose_engine(const acg_dfa* a, int anchored, int earliest, int other, bool strict) {
+  const bool pf_ok = a->pf.supported && !anchored && !(earliest && a->h.match_kind != ACG_STANDARD);
+  const int forced = a->engine_override;
+  if (forced == other) return other;
+  if (forced == ACG_ENGINE_PREFILTER && !pf_ok && strict) return ACG_E_INVALID_ARG;
+  return pf_ok ? ACG_ENGINE_PREFILTER : other;
 }
 
 struct DeviceGuard {
@@ -1467,6 +1499,29 @@ struct DevOut {
   uint64_t offset_add = 0;
 };
 
+// The overlapping search of [span_start, span_end): engine, placement, the walk or prefilter scan, leaving
+// r->n ordered tuples; *first = the number of them that end at or before `min_end`.
+int scan_overlapping(const acg_dfa* a, const uint8_t* hay, bool on_device, uint64_t hay_len, uint64_t span_start,
+                     uint64_t span_end, bool strict, uint64_t min_end, TupleResult* r, uint64_t* first) {
+  Workspace& w = cur_ws();
+  *first = 0;
+  const int engine = choose_engine(a, 0, 0, ACG_ENGINE_WALK, strict);
+  if (engine < 0) return engine;
+  w.stats.engine = engine;
+  Placement pl;
+  int rc = place_input(a, hay, on_device, hay_len, span_start, span_end, engine == ACG_ENGINE_PREFILTER, &pl);
+  if (rc) return rc;
+  if (engine == ACG_ENGINE_PREFILTER) rc = run_prefilter(a, pl.base, pl.readable, span_start, span_end, 0, r, pl.h_src);
+  else rc = run_walk_overlapping(a, pl.base, pl.readable, span_start, span_end, r);
+  if (rc || r->n == 0 || min_end <= span_start) return rc;
+  const uint64_t bound_key = (min_end - span_start + 1) << acb::kTieBits;  // first key with end > min_end
+  CK(acb::launch_lower_bound(w.d_keys[r->sorted_buf], r->n, bound_key, w.d_counter, w.stream));
+  CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  *first = *w.h_counter;
+  return ACG_OK;
+}
+
 int overlapping_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                      uint64_t span_start, uint64_t span_end, int anchored, acg_match* out,
                      uint64_t cap, uint64_t* n_out, uint64_t* fnv, float* kernel_ms,
@@ -1485,35 +1540,15 @@ int overlapping_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, u
   DeviceGuard guard(a->device);
   WsLease lease(a);
   if (lease.rc) return lease.rc;
-  int engine = a->engine_override;
-  if (engine == ACG_ENGINE_PREFILTER && !a->pf.supported) return ACG_E_INVALID_ARG;
-  if (engine != ACG_ENGINE_WALK && engine != ACG_ENGINE_PREFILTER)
-    engine = a->pf.supported ? ACG_ENGINE_PREFILTER : ACG_ENGINE_WALK;
-  cur_ws().stats.engine = engine;
-  const uint8_t* d_base = hay;
-  uint64_t readable = hay_len;
-  const bool pipelined = !hay_on_device && engine == ACG_ENGINE_PREFILTER;
-  if (!hay_on_device) {
-    if ((rc = stage_host_span(a, hay, span_start, span_end, &d_base, pipelined))) return rc;
-    readable = span_end + 32;  // the staging buffer has slack behind the span
-  }
+  // devout: keep the matches on the device, drop ends <= min_end (owned by the previous shard), expand
   TupleResult r;
-  if (engine == ACG_ENGINE_PREFILTER)
-    rc = run_prefilter(a, d_base, readable, span_start, span_end, 0, &r, pipelined ? hay : nullptr);
-  else rc = run_walk_overlapping(a, d_base, readable, span_start, span_end, &r);
-  if (rc) return rc;
+  uint64_t first = 0;
+  if ((rc = scan_overlapping(a, hay, hay_on_device, hay_len, span_start, span_end, true, devout ? devout->min_end : 0,
+                             &r, &first)))
+    return rc;
   if (kernel_ms) *kernel_ms = cur_ws().stats.scan_ms + cur_ws().stats.order_ms;
   if (devout) {
-    // keep the matches on the device: drop ends <= min_end (owned by the previous shard), expand
     Workspace& w = cur_ws();
-    uint64_t first = 0;
-    if (r.n && devout->min_end > span_start) {
-      const uint64_t bound_key = (devout->min_end - span_start + 1) << acb::kTieBits;  // first key with end > min_end
-      CK(acb::launch_lower_bound(w.d_keys[r.sorted_buf], r.n, bound_key, w.d_counter, w.stream));
-      CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream));
-      CK(cudaStreamSynchronize(w.stream));
-      first = *w.h_counter;
-    }
     const uint64_t kept = r.n - first;
     *n_out = kept;
     if (kept > cap) return ACG_E_OVERFLOW;
@@ -1581,35 +1616,10 @@ int sharded_begin(const acg_dfa* a, acg_comm* c, const uint8_t* hay, bool hay_on
   if (lease.rc) return lease.rc;  // (a rank that cannot even get a stream cannot join the exchange either)
   if (covered && own_hi > own_lo) {
     // the local scan, in local offsets: span [read_lo, own_hi) - hay_off
+    // an unusable prefilter override falls back to the walk; ends <= own_lo belong to the previous rank
     lspan_s = read_lo - hay_off;
-    const uint64_t lspan_e = own_hi - hay_off;
-    int engine = a->engine_override;
-    if (engine == ACG_ENGINE_PREFILTER && !a->pf.supported) engine = ACG_ENGINE_AUTO;
-    if (engine != ACG_ENGINE_WALK && engine != ACG_ENGINE_PREFILTER)
-      engine = a->pf.supported ? ACG_ENGINE_PREFILTER : ACG_ENGINE_WALK;
-    cur_ws().stats.engine = engine;
-    const uint8_t* d_base = hay;
-    uint64_t readable = hay_len;
-    const bool pipelined = !hay_on_device && engine == ACG_ENGINE_PREFILTER;
-    if (!hay_on_device) {
-      rc = stage_host_span(a, hay, lspan_s, lspan_e, &d_base, pipelined);
-      readable = lspan_e + 32;
-    }
-    if (!rc) {
-      if (engine == ACG_ENGINE_PREFILTER)
-        rc = run_prefilter(a, d_base, readable, lspan_s, lspan_e, 0, &r, pipelined ? hay : nullptr);
-      else rc = run_walk_overlapping(a, d_base, readable, lspan_s, lspan_e, &r);
-    }
-    if (!rc && r.n && own_lo > read_lo) {
-      // ends <= own_lo belong to the previous rank: first key with end > own_lo
-      Workspace& w = cur_ws();
-      const uint64_t bound_key = (own_lo - read_lo + 1) << acb::kTieBits;
-      cudaError_t e = acb::launch_lower_bound(w.d_keys[r.sorted_buf], r.n, bound_key, w.d_counter, w.stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(w.stream);
-      if (e != cudaSuccess) { cudaGetLastError(); rc = ACG_E_CUDA; }
-      else first = *w.h_counter;
-    }
+    rc = scan_overlapping(a, hay, hay_on_device, hay_len, lspan_s, own_hi - hay_off, false, own_lo - hay_off, &r,
+                          &first);
   }
   if (!covered) rc = ACG_E_INVALID_SPAN;
   // a failed rank still joins the exchange (with the error flag in the top bit) so that nobody hangs
@@ -1724,20 +1734,14 @@ int find_iter_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uin
   DeviceGuard guard(a->device);
   WsLease lease(a);
   if (lease.rc) return lease.rc;
-  int engine = a->engine_override;
-  if (engine == ACG_ENGINE_PREFILTER && (!a->pf.supported || anchored)) return ACG_E_INVALID_ARG;
-  if (engine != ACG_ENGINE_SEQUENTIAL && engine != ACG_ENGINE_PREFILTER)
-    engine = (a->pf.supported && !anchored) ? ACG_ENGINE_PREFILTER : ACG_ENGINE_SEQUENTIAL;
+  const int engine = choose_engine(a, anchored, 0, ACG_ENGINE_SEQUENTIAL, true);
+  if (engine < 0) return engine;
   cur_ws().stats.engine = engine;
-  const uint8_t* d_base = hay;
-  uint64_t readable = hay_len;
-  const bool pipelined = !hay_on_device && engine == ACG_ENGINE_PREFILTER;
-  if (!hay_on_device) {
-    if ((rc = stage_host_span(a, hay, span_start, span_end, &d_base, pipelined))) return rc;
-    readable = span_end + 32;
-  }
+  Placement pl;
+  if ((rc = place_input(a, hay, hay_on_device, hay_len, span_start, span_end, engine == ACG_ENGINE_PREFILTER, &pl)))
+    return rc;
   if (engine == ACG_ENGINE_SEQUENTIAL) {
-    rc = run_seq(a, d_base, span_start, span_end, anchored, 0, 0, out, cap, n_out);
+    rc = run_seq(a, pl.base, span_start, span_end, anchored, 0, 0, out, cap, n_out);
     if (kernel_ms) *kernel_ms = cur_ws().stats.scan_ms;
     return rc;
   }
@@ -1745,8 +1749,7 @@ int find_iter_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uin
   // leftmost kinds: best match per start offset ordered by start, then the same greedy choice.
   const int mode = a->h.match_kind == ACG_STANDARD ? 0 : 1;
   TupleResult r;
-  if ((rc = run_prefilter(a, d_base, readable, span_start, span_end, mode == 0 ? 2 : 1, &r, pipelined ? hay : nullptr)))
-    return rc;
+  if ((rc = run_prefilter(a, pl.base, pl.readable, span_start, span_end, mode == 0 ? 2 : 1, &r, pl.h_src))) return rc;
   if ((rc = run_chain(a, mode, &r))) return rc;
   if (kernel_ms) *kernel_ms = cur_ws().stats.scan_ms + cur_ws().stats.order_ms;
   return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, mode);
@@ -1776,20 +1779,15 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if ((rc = check_start(a->h, anchored))) return rc;
   if (!a->on_device) return ACG_E_NO_DEVICE;
   if (n_docs == 0) return ACG_OK;
-  const bool leftmost = a->h.match_kind != ACG_STANDARD;
-  // find: acg_find's packed-prefilter rule (an unanchored leftmost try_find returns the prefilter's confirmed
-  // leftmost match, src/automaton.rs:1304-1309) and its engine rule (`earliest` on a leftmost automaton
-  // reports the first match state entered, which the per-start scan does not model)
-  if (earliest && !anchored && leftmost && a->h.prefilter_kind == ACG_PRE_PACKED) earliest = 0;
-  const bool pf_ok = a->pf.supported && !anchored && !(earliest && leftmost);
-  const int engine = a->engine_override;
-  if (engine == ACG_ENGINE_PREFILTER && !pf_ok) return ACG_E_INVALID_ARG;
-  const bool use_pf = engine != ACG_ENGINE_SEQUENTIAL && pf_ok;
+  earliest = find_earliest(a, anchored, earliest);
+  const int engine = choose_engine(a, anchored, earliest, ACG_ENGINE_SEQUENTIAL, true);
+  if (engine < 0) return engine;
+  const bool use_pf = engine == ACG_ENGINE_PREFILTER;
   DeviceGuard guard(a->device);
   WsLease lease(a);
   if (lease.rc) return lease.rc;
   Workspace& w = cur_ws();
-  w.stats.engine = use_pf ? ACG_ENGINE_PREFILTER : ACG_ENGINE_SEQUENTIAL;
+  w.stats.engine = engine;
   const uint64_t span_start = offs[0], span_end = offs[n_docs], nd1 = n_docs + 1;
   if ((rc = ensure_docs(w, nd1))) return rc;
   if (what == kBatchFind && (rc = ensure_seq(w, n_docs))) return rc;  // the records, at index doc
@@ -1797,13 +1795,8 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(w.d_docs + w.docs_cap);
   unsigned long long* d_incl = d_counts + w.docs_cap;
   CK(cudaMemcpyAsync(d_offs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
-  const uint8_t* d_base = hay;
-  uint64_t readable = hay_len;
-  const bool pipelined = !hay_on_device && use_pf;
-  if (!hay_on_device) {
-    if ((rc = stage_host_span(a, hay, span_start, span_end, &d_base, pipelined))) return rc;
-    readable = span_end + 32;
-  }
+  Placement pl;
+  if ((rc = place_input(a, hay, hay_on_device, hay_len, span_start, span_end, use_pf, &pl))) return rc;
   auto fetch_per_doc = [&]() -> int {
     CK(cudaMemcpyAsync(flags, w.d_doc_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
     if (what == kBatchFind) CK(cudaMemcpyAsync(out, w.d_seq, n_docs * 24, cudaMemcpyDeviceToHost, w.stream));
@@ -1814,7 +1807,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if (!use_pf) {
     // one thread per document: count, inclusive scan, fill at each document's offset
     acb::SeqDocsLaunch p{};
-    p.hay = d_base;
+    p.hay = pl.base;
     p.doc_offsets = d_offs;
     p.n_docs = n_docs;
     p.anchored = anchored;
@@ -1840,17 +1833,10 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     }
     p.counts = d_counts;
     CK(acb::launch_seq_docs(a->dev, p, w.stream));
-    size_t tb = 0;
-    CK(acb::inclusive_sum_u64(nullptr, tb, d_counts, d_incl, n_docs, w.stream));
-    if (tb > w.temp3_bytes) {
-      cudaFree(w.d_temp3);
-      w.d_temp3 = nullptr;
-      w.temp3_bytes = 0;
-      CK(cudaMalloc(&w.d_temp3, tb));
-      w.temp3_bytes = tb;
-    }
-    tb = w.temp3_bytes;
-    CK(acb::inclusive_sum_u64(w.d_temp3, tb, d_counts, d_incl, n_docs, w.stream));
+    if ((rc = cub_call(w, [&](void* t, size_t& tb) {
+           return acb::inclusive_sum_u64(t, tb, d_counts, d_incl, n_docs, w.stream);
+         })))
+      return rc;
     CK(cudaMemcpyAsync(w.h_counter, d_incl + n_docs - 1, 8, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaStreamSynchronize(w.stream));
     const uint64_t total = w.h_counter[0];
@@ -1882,8 +1868,8 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   docs.n = n_docs;
   docs.unordered = per_doc;
   TupleResult r;
-  if ((rc = run_prefilter(a, d_base, readable, span_start, span_end, pf_mode, &r, pipelined ? hay : nullptr,
-                          UINT64_MAX, UINT64_MAX, &docs)))
+  if ((rc = run_prefilter(a, pl.base, pl.readable, span_start, span_end, pf_mode, &r, pl.h_src, UINT64_MAX,
+                          UINT64_MAX, &docs)))
     return rc;
   if (per_doc) {
     // is_match: the documents of the tuples.  find: per document, the tuple with the smallest key (mode 1: the
@@ -2287,45 +2273,41 @@ int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t sp
   if ((rc = check_start(a->h, anchored))) return rc;
   if (!a->on_device) return ACG_E_NO_DEVICE;
   if (span_start > span_end) return ACG_OK;
-  // Where the reference attaches its packed (Teddy) prefilter -- leftmost kinds only -- an
-  // unanchored try_find returns what the prefilter reports, a confirmed leftmost match
-  // (Candidate::Match, src/automaton.rs:1304-1309), whether or not `earliest` was asked for.
-  if (earliest && !anchored && a->h.match_kind != ACG_STANDARD && a->h.prefilter_kind == ACG_PRE_PACKED) earliest = 0;
+  earliest = find_earliest(a, anchored, earliest);
   DeviceGuard guard(a->device);
   WsLease lease(a);
   if (lease.rc) return lease.rc;
   Workspace& w = cur_ws();
-  // `earliest` on a leftmost automaton reports the first match STATE entered (src/automaton.rs
-  // :1381-1383), which the per-start formulation does not model: sequential engine.
-  const bool use_pf = a->pf.supported && !anchored && a->engine_override != ACG_ENGINE_SEQUENTIAL &&
-                      !(earliest && a->h.match_kind != ACG_STANDARD);
-  const uint8_t* d_base = nullptr;
-  if (!use_pf) {
-    cur_ws().stats.engine = ACG_ENGINE_SEQUENTIAL;
-    if ((rc = stage_host_span(a, hay, span_start, span_end, &d_base))) return rc;
+  const int engine = choose_engine(a, anchored, earliest, ACG_ENGINE_SEQUENTIAL, false);
+  w.stats.engine = engine;
+  // the prefilter engine's window-by-window copy below only takes the room
+  Placement pl;
+  if ((rc = place_input(a, hay, false, hay_len, span_start, span_end, engine == ACG_ENGINE_PREFILTER, &pl))) return rc;
+  if (engine == ACG_ENGINE_SEQUENTIAL) {
     uint64_t n = 0;
-    rc = run_seq(a, d_base, span_start, span_end, anchored, earliest, 1, out, 1, &n);
+    rc = run_seq(a, pl.base, span_start, span_end, anchored, earliest, 1, out, 1, &n);
     if (rc == ACG_OK && n) *found = 1;
     return rc;
   }
   // The reference's try_find is lazy (it stops reading at the first match, SURVEY.md section
   // 7h); the eager device scan therefore works through geometrically growing windows of start
   // offsets (1 MiB, 16 MiB, 256 MiB, ...), copying only what a window needs.
-  cur_ws().stats.engine = ACG_ENGINE_PREFILTER;
-  if ((rc = stage_host_span(a, hay, span_start, span_end, &d_base, true))) return rc;
   const int mode = a->h.match_kind == ACG_STANDARD ? 0 : 1;
   const uint64_t look = a->h.max_pattern_len + 64;
   uint64_t copied_hi = span_start;
-  auto ensure_copied = [&](uint64_t upto) -> int {
-    upto = std::min(upto, span_end);
+  // Scan the start offsets [lo, hi) and fetch the first tuple (*n: the number of tuples).
+  auto first_in = [&](uint64_t lo, uint64_t hi, uint64_t* key, uint32_t* pid, uint64_t* n) -> int {
+    const uint64_t upto = std::min(hi + look, span_end);
     if (upto > copied_hi) {
-      CK(cudaMemcpyAsync(const_cast<uint8_t*>(d_base) + copied_hi, hay + copied_hi, upto - copied_hi,
+      CK(cudaMemcpyAsync(const_cast<uint8_t*>(pl.base) + copied_hi, hay + copied_hi, upto - copied_hi,
                          cudaMemcpyHostToDevice, w.stream));
       copied_hi = upto;
     }
-    return ACG_OK;
-  };
-  auto first_tuple = [&](const TupleResult& r, uint64_t* key, uint32_t* pid) -> int {
+    TupleResult r;
+    int rc = run_prefilter(a, pl.base, copied_hi == span_end ? span_end + 32 : copied_hi, span_start, span_end,
+                           mode == 0 ? 2 : 1, &r, nullptr, lo, hi);
+    *n = r.n;
+    if (rc || r.n == 0) return rc;
     CK(cudaMemcpyAsync(w.h_counter, w.d_keys[r.sorted_buf], 8, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaMemcpyAsync(w.h_counter + 1, w.d_pids[r.sorted_buf], 4, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaStreamSynchronize(w.stream));
@@ -2333,45 +2315,27 @@ int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t sp
     *pid = uint32_t(w.h_counter[1]);
     return ACG_OK;
   };
-  auto decode = [&](uint64_t key, uint32_t pid) {
-    out->pid = pid;
-    out->_pad = 0;
-    if (mode == 1) {
-      out->start = span_start + (key >> acb::kTieBits);
-      out->end = out->start + (key & acb::kTieMask);
-    } else {
-      out->end = span_start + (key >> acb::kTieBits);
-      out->start = out->end - a->h.pattern_lens[pid];
-    }
-  };
+  const uint32_t* plens = a->h.pattern_lens.data();
   uint64_t lo = span_start, win = 1ull << 20;
   while (lo < span_end) {
     const uint64_t hi = std::min(span_end, lo + win);
-    if ((rc = ensure_copied(hi + look))) return rc;
-    TupleResult r;
-    if ((rc = run_prefilter(a, d_base, copied_hi == span_end ? span_end + 32 : copied_hi, span_start,
-                            span_end, mode == 0 ? 2 : 1, &r, nullptr, lo, hi)))
-      return rc;
-    if (r.n) {
-      uint64_t key;
-      uint32_t pid;
-      if ((rc = first_tuple(r, &key, &pid))) return rc;
-      decode(key, pid);
-      if (mode == 0 && out->end > hi && hi < span_end) {
+    uint64_t key = 0, n = 0;
+    uint32_t pid = 0;
+    if ((rc = first_in(lo, hi, &key, &pid, &n))) return rc;
+    if (n) {
+      const uint64_t end = acb::decode_key(key, pid, mode, span_start, plens).end;
+      if (mode == 0 && end > hi && hi < span_end) {
         // Standard: a match that starts in [hi, end) could still end earlier -- scan those starts
-        const uint64_t hi2 = std::min(span_end, uint64_t(out->end));
-        if ((rc = ensure_copied(hi2 + look))) return rc;
-        TupleResult r2;
-        if ((rc = run_prefilter(a, d_base, copied_hi == span_end ? span_end + 32 : copied_hi, span_start,
-                                span_end, mode == 0 ? 2 : 1, &r2, nullptr, hi, hi2)))
-          return rc;
-        if (r2.n) {
-          uint64_t key2;
-          uint32_t pid2;
-          if ((rc = first_tuple(r2, &key2, &pid2))) return rc;
-          if (key2 < key) decode(key2, pid2);
-        }
+        uint64_t key2 = 0, n2 = 0;
+        uint32_t pid2 = 0;
+        if ((rc = first_in(hi, std::min(span_end, end), &key2, &pid2, &n2))) return rc;
+        if (n2 && key2 < key) { key = key2; pid = pid2; }
       }
+      const acb::MatchSpan m = acb::decode_key(key, pid, mode, span_start, plens);
+      out->pid = pid;
+      out->_pad = 0;
+      out->start = m.start;
+      out->end = m.end;
       *found = 1;
       return ACG_OK;
     }

@@ -18,6 +18,18 @@ constexpr int kTieBits = 24;
 constexpr uint64_t kTieMask = (1ull << kTieBits) - 1;
 constexpr uint64_t kInvalidKey = ~0ull;
 
+// (start, end) in haystack offsets of tuple (key, pid) of a search of the span from span_start.  Key
+// layouts (ChainLaunch::mode): 1 = start_rel << 24 | len, otherwise end_rel << 24 | tie.
+struct MatchSpan {
+  uint64_t start, end;
+};
+__host__ __device__ __forceinline__ MatchSpan decode_key(uint64_t key, uint32_t pid, int key_mode, uint64_t span_start,
+                                                         const uint32_t* pattern_lens) {
+  const uint64_t at = span_start + (key >> kTieBits);
+  if (key_mode == 1) return MatchSpan{at, at + (key & kTieMask)};
+  return MatchSpan{at - pattern_lens[pid], at};
+}
+
 struct DfaDev {
   const uint32_t* trans;          // premultiplied ids, as shipped (src/dfa.rs:92-95)
   const uint8_t* classes;         // [256] byte -> class (src/util/alphabet.rs)
@@ -73,28 +85,14 @@ struct FillLaunch {
 };
 cudaError_t launch_dfa_fill_level(const FillLaunch& f, cudaStream_t s);
 
-// Single-lane restatement of FindIter (src/automaton.rs:857-936) over
-// try_find_fwd (:1259-1420): anchored inputs, automata containing the empty
-// pattern, and tiny spans.  Writes (pid,start,end) triples as 3 x u64.
-struct SeqLaunch {
-  const uint8_t* hay;
-  uint64_t span_start, span_end;
-  int anchored;
-  int match_kind;
-  int earliest;         // for single find
-  int single;           // 1: stop after the first match (AhoCorasick::try_find)
-  uint64_t* out;        // [cap * 3]
-  unsigned long long* counter;
-  uint64_t cap;
-};
-cudaError_t launch_seq_find(const DfaDev& dfa, const SeqLaunch& p, cudaStream_t s);
-
-// The same engine over a batch of documents, one thread per document (acg_*_batch when the
-// prefilter engine does not apply).  Two launches: the count pass (incl == nullptr) fills
-// counts[n_docs] -- or flags[n_docs] for is_match -- and after an inclusive scan of the counts the fill
-// pass writes each document's records at out[incl[doc - 1] * 3] as (pid | doc << 32, start, end) with
-// offsets relative to the document, the acg_doc_match layout.  find: one launch (`find`).  A long
-// document is one thread's walk.
+// Sequential engine: single-lane restatement of FindIter (src/automaton.rs:857-936) over try_find_fwd
+// (:1259-1420) -- anchored inputs, automata containing the empty pattern -- one thread per document.
+// A batch (acg_*_batch when the prefilter engine does not apply) takes two launches: the count pass
+// (incl == nullptr) fills counts[n_docs] -- or flags[n_docs] for is_match -- and after an inclusive scan
+// of the counts the fill pass writes each document's records at out[incl[doc - 1] * 3] as
+// (pid | doc << 32, start, end) with offsets relative to the document, the acg_doc_match layout.
+// find: one launch (`find`).  A single document (a single-haystack search) takes one launch: the count
+// pass given `out` also writes the records, from index 0.  A long document is one thread's walk.
 struct SeqDocsLaunch {
   const uint8_t* hay;
   const uint64_t* doc_offsets;  // [n_docs + 1], haystack offsets
@@ -109,7 +107,7 @@ struct SeqDocsLaunch {
   unsigned long long* counts;   // count pass: [n_docs]
   uint8_t* flags;               // count pass, is_match / find: [n_docs] instead of counts
   const unsigned long long* incl;   // fill pass: [n_docs] inclusive scan of counts
-  uint64_t* out;
+  uint64_t* out;                // [cap * 3]; nullptr in the count pass of a batch
   uint64_t cap;                 // records
 };
 cudaError_t launch_seq_docs(const DfaDev& dfa, const SeqDocsLaunch& p, cudaStream_t s);

@@ -4,9 +4,8 @@
 //                                 loop of try_find_overlapping_fwd_imp
 //                                 (src/automaton.rs:1491-1534) + DFA::next_state
 //                                 (src/dfa.rs:218-226) + match expansion (:275-286)
-//   Kseq seq_find_kernel          single-lane FindIter/try_find (anchored inputs,
-//                                 empty-pattern automata)
-//        seq_docs_kernel          the same per document of a batch, one thread each
+//   Kseq seq_docs_kernel          single-lane FindIter/try_find (anchored inputs,
+//                                 empty-pattern automata), one thread per document
 //        doc_flags_kernel         per-document is_match / first match of a batch's
 //        doc_first_kernel         prefilter tuples
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
@@ -250,13 +249,6 @@ __device__ __forceinline__ unsigned long long seq_overlapping(const DfaDev& d, c
   return n;
 }
 
-__global__ void seq_find_kernel(DfaDev d, SeqLaunch p) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const bool earliest = p.match_kind == 0 || p.earliest != 0;
-  *p.counter = seq_find_iter(d, p.hay, p.span_start, p.span_end, p.anchored != 0, earliest, p.single != 0, p.out, 0,
-                             p.cap, 0, 0);
-}
-
 struct SumOp {
   __device__ __forceinline__ unsigned long long operator()(unsigned long long a, unsigned long long b) const { return a + b; }
 };
@@ -265,7 +257,8 @@ struct SumOp {
 // matches, or flags[doc] = (a match exists) when flags is given.  Fill pass: the document's records from
 // index incl[doc - 1] (the matches of the documents before it) on, tagged with the document
 // (doc << 32 in the pid word, offsets relative to the document's first byte).  find: the count pass with
-// flags, the document's one record written at index doc.
+// flags, the document's one record written at index doc.  A count pass given `out` writes from index 0 (one
+// document).
 constexpr int kSeqDocThreads = 128;
 template <bool OVERLAPPING>
 __global__ void __launch_bounds__(kSeqDocThreads) seq_docs_kernel(DfaDev d, SeqDocsLaunch p) {
@@ -273,7 +266,7 @@ __global__ void __launch_bounds__(kSeqDocThreads) seq_docs_kernel(DfaDev d, SeqD
   if (doc >= p.n_docs) return;
   const uint64_t lo = p.doc_offsets[doc], hi = p.doc_offsets[doc + 1];
   const bool fill = p.incl != nullptr;
-  uint64_t* out = fill || p.find ? p.out : nullptr;
+  uint64_t* out = p.out;
   const unsigned long long first = p.find ? doc : (fill && doc ? p.incl[doc - 1] : 0);
   const uint64_t tag = doc << 32;
   if (p.find) {  // the record of "no match", overwritten by the match if there is one
@@ -315,11 +308,9 @@ __device__ __forceinline__ uint64_t doc_of(const uint64_t* offs, uint64_t n_docs
   return lo - 1;
 }
 
-// The haystack start offset of tuple i (key as ChainLaunch::mode: 1 = start_rel << 24 | len,
-// 0 = end_rel << 24 | tie).
-__device__ __forceinline__ uint64_t tuple_start(const DocFlagsLaunch& f, uint64_t i) {
-  const uint64_t key = f.keys[i];
-  return f.span_start + (f.mode == 1 ? key >> kTieBits : (key >> kTieBits) - f.pattern_lens[f.pids[i]]);
+// The haystack offsets of tuple i.
+__device__ __forceinline__ MatchSpan tuple_span(const DocFlagsLaunch& f, uint64_t i) {
+  return decode_key(f.keys[i], f.pids[i], f.mode, f.span_start, f.pattern_lens);
 }
 
 // Over the n tuples of a prefilter scan.  is_match: flags[doc] = 1 for the document of every tuple.
@@ -327,7 +318,7 @@ __device__ __forceinline__ uint64_t tuple_start(const DocFlagsLaunch& f, uint64_
 __global__ void doc_flags_kernel(DocFlagsLaunch f) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= f.n) return;
-  const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, tuple_start(f, i));
+  const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, tuple_span(f, i).start);
   if (f.best) atomicMin(f.best + doc, (unsigned long long)f.keys[i]);
   else f.flags[doc] = 1;
 }
@@ -349,15 +340,13 @@ __global__ void doc_first_clear_kernel(DocFlagsLaunch f) {
 __global__ void doc_first_kernel(DocFlagsLaunch f) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= f.n) return;
-  const uint64_t s = tuple_start(f, i);
-  const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, s);
-  const uint64_t key = f.keys[i];
-  if (key != f.best[doc]) return;
-  const uint32_t pid = f.pids[i];
+  const MatchSpan m = tuple_span(f, i);
+  const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, m.start);
+  if (f.keys[i] != f.best[doc]) return;
   const uint64_t base = f.doc_offsets[doc];
-  f.out[doc * 3 + 0] = (uint64_t)pid | doc << 32;
-  f.out[doc * 3 + 1] = s - base;
-  f.out[doc * 3 + 2] = s + (f.mode == 1 ? key & kTieMask : f.pattern_lens[pid]) - base;
+  f.out[doc * 3 + 0] = (uint64_t)f.pids[i] | doc << 32;
+  f.out[doc * 3 + 1] = m.start - base;
+  f.out[doc * 3 + 2] = m.end - base;
   f.flags[doc] = 1;
 }
 
@@ -374,12 +363,11 @@ __global__ void __launch_bounds__(kExpandThreads) expand_kernel(ExpandLaunch e) 
   for (uint64_t base = (uint64_t)blockIdx.x * kExpandThreads; base < m; base += (uint64_t)gridDim.x * kExpandThreads) {
     const uint64_t i = base + threadIdx.x;
     if (i < m) {
-      const uint64_t key = e.keys[e.first + i];
       const uint32_t pid = e.pids[e.first + i];
-      const uint64_t end = e.span_start + (key >> kTieBits) + e.offset_add;
+      const MatchSpan span = decode_key(e.keys[e.first + i], pid, 0, e.span_start + e.offset_add, e.pattern_lens);
       s_rec[threadIdx.x * 3 + 0] = (uint64_t)pid;
-      s_rec[threadIdx.x * 3 + 1] = end - e.pattern_lens[pid];
-      s_rec[threadIdx.x * 3 + 2] = end;
+      s_rec[threadIdx.x * 3 + 1] = span.start;
+      s_rec[threadIdx.x * 3 + 2] = span.end;
     }
     __syncthreads();
     const uint64_t cnt = m - base < kExpandThreads ? m - base : kExpandThreads;  // records of this block
@@ -441,12 +429,6 @@ cudaError_t launch_dfa_fill_level(const FillLaunch& f, cudaStream_t s) {
 #endif
   const uint64_t blocks = ((uint64_t)f.n * 32 + kFillThreads - 1) / kFillThreads;
   ACB_LAUNCH(dfa_fill_level_kernel, (unsigned)blocks, kFillThreads, 0, s, f);
-  return cudaGetLastError();
-}
-
-
-cudaError_t launch_seq_find(const DfaDev& dfa, const SeqLaunch& p, cudaStream_t s) {
-  ACB_LAUNCH(seq_find_kernel, 1, 32, 0, s, dfa, p);
   return cudaGetLastError();
 }
 
