@@ -48,6 +48,11 @@ __device__ __forceinline__ void tma_load_1d(uint32_t smem_dst, const void* gmem_
                ::"r"(smem_dst), "l"(gmem_src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// cp.async.bulk.prefetch.L2 (SASS UBLKPF): bring `bytes` (multiple of 16) of 16-byte aligned global
+// memory into L2 ahead of the bulk copy that will read them; no shared memory, no completion.
+__device__ __forceinline__ void bulk_prefetch_l2(const void* gmem_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem_src), "r"(bytes) : "memory");
+}
 
 // ---- shared-memory reads by shared address (volatile: they stay behind the mbarrier wait) ----
 __device__ __forceinline__ uint4 lds128(uint32_t a) {
