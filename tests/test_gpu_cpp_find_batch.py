@@ -1,5 +1,6 @@
 """tests/cpp/test_find_batch.cpp (find_batch / try_find_batch of include/acb200.hpp) on the GPU; and, without a
-GPU, the same program linked against the dry-run library of tests/emu/."""
+GPU, the same program linked against the dry-run library of tests/emu/.  The executables go to the test's
+temporary directory: the repository tree may be read-only."""
 import subprocess
 import sys
 from pathlib import Path
@@ -19,12 +20,12 @@ def _build_and_run(exe, libdir, libname):
 
 
 @pytest.mark.gpu
-def test_cpp_find_batch_runs():
-    _build_and_run(CPP / "test_find_batch", ROOT / "aho-corasick_b200", "acb200")
+def test_cpp_find_batch_runs(tmp_path):
+    _build_and_run(tmp_path / "test_find_batch", ROOT / "aho-corasick_b200", "acb200")
 
 
-def test_cpp_find_batch_on_the_dry_run_library():
+def test_cpp_find_batch_on_the_dry_run_library(tmp_path):
     sys.path.insert(0, str(ROOT / "tests" / "emu"))
     import build_emu
     lib = build_emu.build()
-    _build_and_run(CPP / "test_find_batch_emu", lib.parent, "acb200_emu")
+    _build_and_run(tmp_path / "test_find_batch_emu", lib.parent, "acb200_emu")

@@ -1,59 +1,15 @@
-"""Switchable kernel / plan variants (include/acb200_debug.h: ACG_EXP_KEY24, ACG_EXP_STATIC_TILES)
-on the device: same tuple stream as the oracle and as the default kernel; and the dense table built
-on the device."""
-import ctypes
-
+"""The dense table built on the device (acg_build_on_device) against the host builder's, and searched
+by both engines.  The switchable kernel variants (include/acb200_debug.h: ACG_EXP_KEY24,
+ACG_EXP_STATIC_TILES, ACG_EXP_GLOBAL_TILES) are rows of tests/test_gpu_kernel_matrix.py."""
 import numpy as np
 import pytest
 
 import aho_corasick_b200 as ab
 import oracle_py as O
 from aho_corasick_b200 import workload as W
-from test_gpu_parity import assert_np_equal, build, to_device
+from test_gpu_parity import assert_np_equal, to_device
 
 pytestmark = pytest.mark.gpu
-
-
-def set_experiment(ac, flags):
-    ab._lib.acg_debug_set_experiment.argtypes = [ctypes.c_void_p, ctypes.c_uint32]
-    assert ab._lib.acg_debug_set_experiment(ac._h, flags) == 0
-    return ac
-
-
-@pytest.mark.timeout(600)
-@pytest.mark.parametrize("flags", [8, 16, 32, 40])
-@pytest.mark.parametrize("cfg,kind,ci", [("cfg2", 0, False), ("cfg3", 1, True)])
-def test_experimental_prefilter_variants(cfg, kind, ci, flags):
-    import torch
-    n = 24 << 20
-    pats = W.make_patterns(W.CONFIGS[cfg]["n_patterns"], W.CONFIGS[cfg]["pattern_seed"])
-    t = torch.empty(n, dtype=torch.uint8)
-    W.torch_fill_config(cfg, t, pats, chunk=1 << 24)
-    hay = t.numpy()
-    ac = set_experiment(build(pats, kind, ascii_case_insensitive=ci, kind=ab.AhoCorasickKind.DFA), flags)
-    o = O.Oracle(pats, match_kind=kind, ascii_case_insensitive=ci, kind=O.KIND_DFA)
-    d = to_device(t)
-    if kind == 0:
-        want = o.find_overlapping_iter_np(hay)
-        got, _ = ac.find_overlapping_iter_dev_np(d.data_ptr(), n)
-        assert_np_equal(got, want, (cfg, flags))
-        assert ac.last_stats()["engine"] == int(ab.Engine.Prefilter)
-        cand = ac.last_stats()["candidates"]
-        # unaligned span, odd span end
-        s, e = 4099, n - 777
-        sub, _ = ac.find_overlapping_iter_dev_np(d.data_ptr(), n, span=(s, e))
-        assert_np_equal(sub, o.find_overlapping_iter_np(hay, span=(s, e)), (cfg, flags, "span"))
-        # the filter is the same: the default kernel verifies as many candidates, give or take the
-        # unconditional ones (hits that own the start one byte before a tile depend on the tiling)
-        set_experiment(ac, flags & 8)
-        ac.find_overlapping_iter_dev_np(d.data_ptr(), n)
-        if not flags & 8:   # (27-bit first-stage keys are a different filter)
-            assert abs(ac.last_stats()["candidates"] - cand) <= cand // 10
-    else:
-        want = o.find_iter_np(hay)
-        got, _ = ac.find_iter_dev_np(d.data_ptr(), n)
-        assert_np_equal(got, want, (cfg, flags))
-        assert_np_equal(ac.try_find_iter_np(hay), want, (cfg, flags, "host"))
 
 
 @pytest.mark.timeout(900)
