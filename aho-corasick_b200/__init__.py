@@ -9,6 +9,7 @@ Python is test/bench glue only: the product is the shared library.
 """
 from __future__ import annotations
 
+import collections
 import ctypes as C
 import enum
 from pathlib import Path
@@ -154,6 +155,10 @@ def _declare(lib):
     lib.acg_find_overlapping_batch.argtypes = lib.acg_find_iter_batch.argtypes
     lib.acg_is_match_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _vp]
     lib.acg_find_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _i, _vp, _vp]
+    lib.acg_find_iter_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _vp, _u64, _vp, C.POINTER(_u64)]
+    lib.acg_find_overlapping_batch_devout.argtypes = lib.acg_find_iter_batch_devout.argtypes
+    lib.acg_is_match_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _vp]
+    lib.acg_find_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _i, _vp, _vp]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -226,16 +231,21 @@ def _hay_ptr(hay):
     return arr, arr.ctypes.data if arr.size else 0, arr.size
 
 
+def _host_offsets(offsets):
+    """[n_docs + 1] CSR bounds in host memory as a uint64 ndarray."""
+    offs = np.ascontiguousarray(offsets, dtype=np.int64)
+    if offs.ndim != 1 or offs.size == 0 or (offs < 0).any():
+        raise ValueError("document offsets must be a non-empty 1-D array of non-negative integers")
+    return offs.astype(np.uint64)
+
+
 def _batch_input(docs):
     """(keepalive, address, length, on_device, uint64 offsets) of a batch of documents: a list of
     bytes / str, or a (values, offsets) pair -- values a contiguous uint8 ndarray or a CUDA torch.uint8
     tensor, offsets the [n_docs + 1] CSR bounds (host, int64)."""
     if isinstance(docs, tuple) and len(docs) == 2:
         values, offsets = docs
-        offs = np.ascontiguousarray(offsets, dtype=np.int64)
-        if offs.ndim != 1 or offs.size == 0 or (offs < 0).any():
-            raise ValueError("document offsets must be a non-empty 1-D array of non-negative integers")
-        offs = offs.astype(np.uint64)
+        offs = _host_offsets(offsets)
         if getattr(values, "is_cuda", False):
             if str(values.dtype) != "torch.uint8" or not values.is_contiguous():
                 raise TypeError("device haystack must be a contiguous torch.uint8 tensor")
@@ -248,6 +258,45 @@ def _batch_input(docs):
         np.cumsum(np.fromiter(map(len, pieces), dtype=np.uint64, count=len(pieces)), out=offs[1:])
     keep, ptr, n = _hay_ptr(b"".join(pieces))
     return keep, ptr, n, 0, offs
+
+
+def _devout_offsets(offsets, n_docs):
+    """(keepalive, address, n_docs, on_device) of the offsets of a raw-pointer devout call: a host array of
+    [n_docs + 1] bounds, or an int device address of them with n_docs given."""
+    if isinstance(offsets, int):
+        if n_docs is None:
+            raise TypeError("offsets given as a device address need n_docs")
+        return None, offsets, int(n_docs), 1
+    offs = _host_offsets(offsets)
+    return offs, offs.ctypes.data, offs.size - 1, 0
+
+
+def _torch_batch(docs):
+    """(values, offsets keepalive, offsets address, n_docs, on_device) of a (CUDA torch.uint8 values, offsets)
+    batch, offsets an int64 CUDA tensor on the values' device or a host array.  Torch's current stream is
+    synchronised first: the library runs on its own streams and the inputs may still be in flight."""
+    import torch
+    values, offsets = docs
+    if not getattr(values, "is_cuda", False) or values.dtype != torch.uint8 or not values.is_contiguous():
+        raise TypeError("values must be a contiguous CUDA torch.uint8 tensor")
+    if isinstance(offsets, torch.Tensor) and offsets.is_cuda:
+        if offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() == 0:
+            raise ValueError("device document offsets must be a non-empty 1-D int64 tensor")
+        if offsets.device != values.device:
+            raise ValueError("document offsets must be on the haystack's device")
+        offsets = offsets.contiguous()
+        keep, ptr, n_docs, on_dev = offsets, offsets.data_ptr(), offsets.numel() - 1, 1
+    else:
+        keep, ptr, n_docs, on_dev = _devout_offsets(offsets, None)
+    torch.cuda.current_stream(values.device).synchronize()
+    return values, keep, ptr, n_docs, on_dev
+
+
+# Device-resident batch records (find_iter_batch_torch / find_overlapping_iter_batch_torch), CUDA tensors on the
+# haystack's device: `records` int64 [n, 3], the acg_doc_match words (pid | doc << 32, start, end); `offsets` int64
+# [n_docs + 1], the records of document d are records[offsets[d]:offsets[d + 1]]; `pid`, `doc` [n] derived from
+# records[:, 0], `start`, `end` views of its other columns.
+BatchMatches = collections.namedtuple("BatchMatches", "records offsets pid doc start end")
 
 
 def _span(span, n):
@@ -727,6 +776,103 @@ class AhoCorasick:
         found, r = self.find_batch_np(docs, anchored, earliest)
         return [Match(p, s, e) if f else None
                 for f, p, s, e in zip(found.tolist(), r["pid"].tolist(), r["start"].tolist(), r["end"].tolist())]
+
+    # ---- batched search with device-resident results (acg_*_batch_devout) ----
+    # Raw-pointer forms: d_hay_ptr / out_ptr / match_offsets_ptr / flags_ptr / found_ptr are device addresses;
+    # `offsets` is a host array of [n_docs + 1] bounds, or an int device address of them with `n_docs` given.
+    def _batch_devout(self, fn, d_hay_ptr, hay_len, offsets, out_ptr, cap, match_offsets_ptr, anchored, n_docs):
+        keep, optr, n_docs, on_dev = _devout_offsets(offsets, n_docs)
+        cnt = _u64()
+        rc = fn(self._h, d_hay_ptr, hay_len, optr, on_dev, n_docs, int(anchored), out_ptr, cap, match_offsets_ptr,
+                C.byref(cnt))
+        if rc == E_OVERFLOW:
+            raise OverflowError(int(cnt.value))
+        if rc:
+            self._raise(rc)
+        return int(cnt.value)
+
+    def find_iter_batch_devout(self, d_hay_ptr, hay_len, offsets, out_ptr, cap, match_offsets_ptr,
+                               anchored=Anchored.No, n_docs=None):
+        """find_iter of every document into device memory: acg_doc_match records at out_ptr and their CSR index
+        by document ([n_docs + 1] uint64) at match_offsets_ptr.  Returns the record count; raises
+        OverflowError(needed) if cap is too small (nothing is written then)."""
+        return self._batch_devout(_lib.acg_find_iter_batch_devout, d_hay_ptr, hay_len, offsets, out_ptr, cap,
+                                  match_offsets_ptr, anchored, n_docs)
+
+    def find_overlapping_iter_batch_devout(self, d_hay_ptr, hay_len, offsets, out_ptr, cap, match_offsets_ptr,
+                                           anchored=Anchored.No, n_docs=None):
+        return self._batch_devout(_lib.acg_find_overlapping_batch_devout, d_hay_ptr, hay_len, offsets, out_ptr, cap,
+                                  match_offsets_ptr, anchored, n_docs)
+
+    def is_match_batch_devout(self, d_hay_ptr, hay_len, offsets, flags_ptr, anchored=Anchored.No, n_docs=None):
+        """is_match of every document: flags_ptr[d] = 0 / 1 (uint8, device)."""
+        keep, optr, n_docs, on_dev = _devout_offsets(offsets, n_docs)
+        rc = _lib.acg_is_match_batch_devout(self._h, d_hay_ptr, hay_len, optr, on_dev, n_docs, int(anchored),
+                                            flags_ptr)
+        if rc:
+            self._raise(rc)
+
+    def find_batch_devout(self, d_hay_ptr, hay_len, offsets, out_ptr, found_ptr, anchored=Anchored.No,
+                          earliest=False, n_docs=None):
+        """try_find of every document: found_ptr[d] (uint8) and the record out_ptr[d] (acg_doc_match), device."""
+        keep, optr, n_docs, on_dev = _devout_offsets(offsets, n_docs)
+        rc = _lib.acg_find_batch_devout(self._h, d_hay_ptr, hay_len, optr, on_dev, n_docs, int(anchored),
+                                        int(earliest), out_ptr, found_ptr)
+        if rc:
+            self._raise(rc)
+
+    # Torch forms: `docs` = (values, offsets), values a CUDA torch.uint8 tensor, offsets an int64 CUDA tensor on
+    # its device or a host array; the results are CUDA tensors on the values' device.
+    def _collect_batch_torch(self, fn, docs, anchored):
+        import torch
+        values, keep, optr, n_docs, on_dev = _torch_batch(docs)
+        match_offsets = torch.empty(n_docs + 1, dtype=torch.int64, device=values.device)
+        cap = self._cap_hint
+        for _ in range(2):
+            records = torch.empty((cap, 3), dtype=torch.int64, device=values.device)
+            cnt = _u64()
+            rc = fn(self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs, int(anchored),
+                    records.data_ptr(), cap, match_offsets.data_ptr(), C.byref(cnt))
+            if rc == E_OVERFLOW:  # retry once with the reported count and room to spare
+                cap = int(cnt.value) + int(cnt.value) // 8 + 64
+                self._cap_hint = max(self._cap_hint, cap)
+                continue
+            if rc:
+                self._raise(rc)
+            r = records[: cnt.value]
+            return BatchMatches(r, match_offsets, r[:, 0] & 0xFFFFFFFF, r[:, 0] >> 32, r[:, 1], r[:, 2])
+        raise DeviceError(E_OVERFLOW)
+
+    def find_iter_batch_torch(self, docs, anchored=Anchored.No):
+        """find_iter of every document, results on the device: a BatchMatches of CUDA tensors."""
+        return self._collect_batch_torch(_lib.acg_find_iter_batch_devout, docs, anchored)
+
+    def find_overlapping_iter_batch_torch(self, docs):
+        return self._collect_batch_torch(_lib.acg_find_overlapping_batch_devout, docs, Anchored.No)
+
+    def is_match_batch_torch(self, docs, anchored=Anchored.No):
+        """is_match of every document: CUDA bool tensor [n_docs]."""
+        import torch
+        values, keep, optr, n_docs, on_dev = _torch_batch(docs)
+        flags = torch.empty(n_docs, dtype=torch.bool, device=values.device)
+        rc = _lib.acg_is_match_batch_devout(self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs,
+                                            int(anchored), flags.data_ptr())
+        if rc:
+            self._raise(rc)
+        return flags
+
+    def find_batch_torch(self, docs, anchored=Anchored.No, earliest=False):
+        """try_find of every document: (found, CUDA bool [n_docs]; records, CUDA int64 [n_docs, 3] acg_doc_match
+        words).  A document without a match has found False and the record (0 | doc << 32, 0, 0)."""
+        import torch
+        values, keep, optr, n_docs, on_dev = _torch_batch(docs)
+        found = torch.empty(n_docs, dtype=torch.bool, device=values.device)
+        records = torch.empty((n_docs, 3), dtype=torch.int64, device=values.device)
+        rc = _lib.acg_find_batch_devout(self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs,
+                                        int(anchored), int(earliest), records.data_ptr(), found.data_ptr())
+        if rc:
+            self._raise(rc)
+        return found, records
 
     # ---- replace / stream: host-side glue over find_iter, as in the reference -------------------
     @staticmethod

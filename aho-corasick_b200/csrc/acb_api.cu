@@ -1757,19 +1757,32 @@ int find_iter_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uin
 
 enum BatchKind { kBatchFindIter = 0, kBatchOverlapping = 1, kBatchIsMatch = 2, kBatchFind = 3 };
 
+// acg_*_batch_devout: the results stay in device memory -- `out` / `flags` are device pointers, and find_iter /
+// overlapping also fill the records' CSR index by document -- and the offsets may be there too.
+struct BatchDevOut {
+  bool offsets_on_device = false;
+  uint64_t* match_offsets = nullptr;  // find_iter / overlapping: [n_docs + 1]
+};
+
 // acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch / acg_find_batch (include/acb200.h).
 // is_match and find give one result per document: flags[n_docs] (find: found) and, for find, out[n_docs].
 int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                const uint64_t* offs, uint64_t n_docs, int anchored, acg_match* out, uint64_t cap, uint64_t* n_out,
-               uint8_t* flags, int earliest = 0) {
+               uint8_t* flags, int earliest = 0, const BatchDevOut* dv = nullptr) {
   const bool per_doc = what == kBatchIsMatch || what == kBatchFind;
   if (!a || !offs || (per_doc ? n_docs && (!flags || (what == kBatchFind && !out)) : !n_out))
     return ACG_E_INVALID_ARG;
+  if (dv && !per_doc && (!dv->match_offsets || (!out && cap))) return ACG_E_INVALID_ARG;
   if (n_out) *n_out = 0;
   if (n_docs >= (1ull << 32)) return ACG_E_INVALID_ARG;
-  for (uint64_t i = 0; i < n_docs; ++i)
-    if (offs[i + 1] < offs[i]) return ACG_E_INVALID_SPAN;
-  if (offs[n_docs] > hay_len) return ACG_E_INVALID_SPAN;
+  const bool offs_on_device = dv && dv->offsets_on_device;
+  if (offs_on_device) {
+    if (reinterpret_cast<uintptr_t>(offs) & 7) return ACG_E_INVALID_ARG;
+  } else {
+    for (uint64_t i = 0; i < n_docs; ++i)
+      if (offs[i + 1] < offs[i]) return ACG_E_INVALID_SPAN;
+    if (offs[n_docs] > hay_len) return ACG_E_INVALID_SPAN;
+  }
   int rc = check_anchored(a->h.start_kind, anchored);
   if (rc) return rc;
   if (what == kBatchOverlapping) {  // Automaton::try_find_overlapping_iter, src/automaton.rs:397-423
@@ -1778,9 +1791,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   }
   if ((rc = check_start(a->h, anchored))) return rc;
   if (!a->on_device) return ACG_E_NO_DEVICE;
-  if (n_docs == 0) return ACG_OK;
+  if (n_docs == 0 && !dv) return ACG_OK;
   earliest = find_earliest(a, anchored, earliest);
-  const int engine = choose_engine(a, anchored, earliest, ACG_ENGINE_SEQUENTIAL, true);
+  const int engine = n_docs ? choose_engine(a, anchored, earliest, ACG_ENGINE_SEQUENTIAL, true) : ACG_ENGINE_SEQUENTIAL;
   if (engine < 0) return engine;
   const bool use_pf = engine == ACG_ENGINE_PREFILTER;
   DeviceGuard guard(a->device);
@@ -1788,18 +1801,44 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if (lease.rc) return lease.rc;
   Workspace& w = cur_ws();
   w.stats.engine = engine;
-  const uint64_t span_start = offs[0], span_end = offs[n_docs], nd1 = n_docs + 1;
+  const uint64_t nd1 = n_docs + 1;
   if ((rc = ensure_docs(w, nd1))) return rc;
-  if (what == kBatchFind && (rc = ensure_seq(w, n_docs))) return rc;  // the records, at index doc
-  uint64_t* d_offs = w.d_docs;
+  if (what == kBatchFind && !dv && (rc = ensure_seq(w, n_docs))) return rc;  // the records, at index doc
+  uint64_t span_start, span_end;
+  const uint64_t* d_offs = w.d_docs;
   unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(w.d_docs + w.docs_cap);
   unsigned long long* d_incl = d_counts + w.docs_cap;
-  CK(cudaMemcpyAsync(d_offs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
+  if (offs_on_device) {
+    // checked where they are; the span bounds come back with the verdict (placement and the scan plan need them)
+    CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
+    CK(acb::launch_check_offsets(offs, n_docs, hay_len, w.d_counter, w.stream));
+    CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 24, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    w.stats.launches += 1;
+    if (w.h_counter[0]) return ACG_E_INVALID_SPAN;
+    span_start = w.h_counter[1];
+    span_end = w.h_counter[2];
+    d_offs = offs;
+  } else {
+    span_start = offs[0];
+    span_end = offs[n_docs];
+    CK(cudaMemcpyAsync(w.d_docs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
+  }
+  if (n_docs == 0) {  // device output: the index of no records
+    if (!per_doc) CK(cudaMemsetAsync(dv->match_offsets, 0, 8, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    return ACG_OK;
+  }
   Placement pl;
   if ((rc = place_input(a, hay, hay_on_device, hay_len, span_start, span_end, use_pf, &pl))) return rc;
+  // per-document results: the caller's device arrays, or the workspace's and a copy to the host
+  uint8_t* d_flags = dv ? flags : w.d_doc_flags;
+  uint64_t* d_find = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq;
   auto fetch_per_doc = [&]() -> int {
-    CK(cudaMemcpyAsync(flags, w.d_doc_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
-    if (what == kBatchFind) CK(cudaMemcpyAsync(out, w.d_seq, n_docs * 24, cudaMemcpyDeviceToHost, w.stream));
+    if (!dv) {
+      CK(cudaMemcpyAsync(flags, w.d_doc_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
+      if (what == kBatchFind) CK(cudaMemcpyAsync(out, w.d_seq, n_docs * 24, cudaMemcpyDeviceToHost, w.stream));
+    }
     CK(cudaStreamSynchronize(w.stream));
     return ACG_OK;
   };
@@ -1817,10 +1856,10 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     p.earliest = what == kBatchIsMatch || earliest;
     CK(cudaEventRecord(w.ev0, w.stream));
     if (per_doc) {
-      p.flags = w.d_doc_flags;
+      p.flags = d_flags;
       if (what == kBatchFind) {
         p.find = 1;
-        p.out = w.d_seq;
+        p.out = d_find;
         p.cap = n_docs;
       }
       CK(acb::launch_seq_docs(a->dev, p, w.stream));
@@ -1846,15 +1885,20 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     if (total > cap) return ACG_E_OVERFLOW;
     if (total) {
       if (!out) return ACG_E_INVALID_ARG;
-      if ((rc = ensure_seq(w, total))) return rc;
+      if (!dv && (rc = ensure_seq(w, total))) return rc;
       p.incl = d_incl;
-      p.out = w.d_seq;
+      p.out = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq;
       p.cap = total;
       CK(acb::launch_seq_docs(a->dev, p, w.stream));
       w.stats.launches += 1;
     }
     CK(cudaEventRecord(w.ev1, w.stream));
-    if (total) CK(cudaMemcpyAsync(out, w.d_seq, total * 24, cudaMemcpyDeviceToHost, w.stream));
+    if (dv) {  // the CSR index is the inclusive scan behind a zero
+      CK(cudaMemsetAsync(dv->match_offsets, 0, 8, w.stream));
+      CK(cudaMemcpyAsync(dv->match_offsets + 1, d_incl, n_docs * 8, cudaMemcpyDeviceToDevice, w.stream));
+    } else if (total) {
+      CK(cudaMemcpyAsync(out, w.d_seq, total * 24, cudaMemcpyDeviceToHost, w.stream));
+    }
     CK(cudaStreamSynchronize(w.stream));
     cudaEventElapsedTime(&ms, w.ev0, w.ev1);
     w.stats.scan_ms = ms;
@@ -1884,15 +1928,15 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     f.span_start = span_start;
     f.doc_offsets = d_offs;
     f.n_docs = n_docs;
-    f.flags = w.d_doc_flags;
+    f.flags = d_flags;
     CK(cudaEventRecord(w.ev2, w.stream));
     if (what == kBatchFind) {
       f.best = d_counts;
-      f.out = w.d_seq;
+      f.out = d_find;
       CK(acb::launch_doc_first(f, w.stream));
       w.stats.launches += 3;
     } else {
-      CK(cudaMemsetAsync(w.d_doc_flags, 0, n_docs, w.stream));
+      CK(cudaMemsetAsync(d_flags, 0, n_docs, w.stream));
       CK(acb::launch_doc_flags(f, w.stream));
       w.stats.launches += 1;
     }
@@ -1903,7 +1947,32 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     return ACG_OK;
   }
   if (what == kBatchFindIter && (rc = run_chain(a, chain_mode, &r))) return rc;
-  return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, chain_mode, offs);
+  if (!dv) return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, chain_mode, offs);
+  *n_out = r.n;
+  if (r.n > cap) return ACG_E_OVERFLOW;  // nothing written: the caller retries with room for *n_out
+  CK(cudaEventRecord(w.ev2, w.stream));
+  if (r.n == 0) {
+    CK(cudaMemsetAsync(dv->match_offsets, 0, nd1 * 8, w.stream));
+  } else {
+    acb::DocRecordsLaunch e;
+    e.keys = w.d_keys[r.sorted_buf];
+    e.pids = w.d_pids[r.sorted_buf];
+    e.pattern_lens = a->d_plens;
+    e.n = r.n;
+    e.mode = chain_mode;
+    e.span_start = span_start;
+    e.doc_offsets = d_offs;
+    e.n_docs = n_docs;
+    e.out = reinterpret_cast<uint64_t*>(out);
+    e.match_offsets = dv->match_offsets;
+    CK(acb::launch_doc_records(e, w.stream));
+    w.stats.launches += 1;
+  }
+  CK(cudaEventRecord(w.ev3, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+  w.stats.order_ms += ms;
+  return ACG_OK;
 }
 
 }  // namespace
@@ -2262,6 +2331,41 @@ int acg_find_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint
                    uint8_t* found) {
   return batch_impl(a, kBatchFind, hay, hay_on_device != 0, hay_len, doc_offsets, n_docs, anchored,
                     reinterpret_cast<acg_match*>(out), n_docs, nullptr, found, earliest != 0);
+}
+
+int acg_find_iter_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len, const uint64_t* doc_offsets,
+                               int offsets_on_device, uint64_t n_docs, int anchored, acg_doc_match* d_out,
+                               uint64_t cap, uint64_t* d_match_offsets, uint64_t* n_out) {
+  BatchDevOut dv;
+  dv.offsets_on_device = offsets_on_device != 0;
+  dv.match_offsets = d_match_offsets;
+  return batch_impl(a, kBatchFindIter, static_cast<const uint8_t*>(d_hay), true, hay_len, doc_offsets, n_docs,
+                    anchored, reinterpret_cast<acg_match*>(d_out), cap, n_out, nullptr, 0, &dv);
+}
+int acg_find_overlapping_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len,
+                                      const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                                      int anchored, acg_doc_match* d_out, uint64_t cap, uint64_t* d_match_offsets,
+                                      uint64_t* n_out) {
+  BatchDevOut dv;
+  dv.offsets_on_device = offsets_on_device != 0;
+  dv.match_offsets = d_match_offsets;
+  return batch_impl(a, kBatchOverlapping, static_cast<const uint8_t*>(d_hay), true, hay_len, doc_offsets, n_docs,
+                    anchored, reinterpret_cast<acg_match*>(d_out), cap, n_out, nullptr, 0, &dv);
+}
+int acg_is_match_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len, const uint64_t* doc_offsets,
+                              int offsets_on_device, uint64_t n_docs, int anchored, uint8_t* d_flags) {
+  BatchDevOut dv;
+  dv.offsets_on_device = offsets_on_device != 0;
+  return batch_impl(a, kBatchIsMatch, static_cast<const uint8_t*>(d_hay), true, hay_len, doc_offsets, n_docs,
+                    anchored, nullptr, 0, nullptr, d_flags, 0, &dv);
+}
+int acg_find_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len, const uint64_t* doc_offsets,
+                          int offsets_on_device, uint64_t n_docs, int anchored, int earliest, acg_doc_match* d_out,
+                          uint8_t* d_found) {
+  BatchDevOut dv;
+  dv.offsets_on_device = offsets_on_device != 0;
+  return batch_impl(a, kBatchFind, static_cast<const uint8_t*>(d_hay), true, hay_len, doc_offsets, n_docs,
+                    anchored, reinterpret_cast<acg_match*>(d_out), n_docs, nullptr, d_found, earliest != 0, &dv);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

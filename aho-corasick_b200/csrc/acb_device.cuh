@@ -135,6 +135,30 @@ cudaError_t launch_doc_flags(const DocFlagsLaunch& f, cudaStream_t s);
 // find: three launches (clear, per-document minimum key, write the minimum's record)
 cudaError_t launch_doc_first(const DocFlagsLaunch& f, cudaStream_t s);
 
+// Device-resident batch results (acg_find_iter_batch_devout / acg_find_overlapping_batch_devout, prefilter
+// engine): the n ordered tuples, document-major, become acg_doc_match records out[i * 3] = (pid | doc << 32,
+// start, end), offsets relative to the document, and match_offsets[d] = the index of document d's first record
+// (match_offsets[n_docs] = n).  Record i writes match_offsets[d] = i for every d in (doc of i - 1, doc of i], the
+// last one also (doc of n - 1, n_docs]: every entry is written once, with no atomics.  n > 0.
+struct DocRecordsLaunch {
+  const uint64_t* keys;
+  const uint32_t* pids;
+  const uint32_t* pattern_lens;
+  uint64_t n;
+  int mode;                     // key layout as ChainLaunch::mode
+  uint64_t span_start;
+  const uint64_t* doc_offsets;  // [n_docs + 1]
+  uint64_t n_docs;
+  uint64_t* out;                // [n * 3]
+  uint64_t* match_offsets;      // [n_docs + 1]
+};
+cudaError_t launch_doc_records(const DocRecordsLaunch& e, cudaStream_t s);
+
+// Offsets in device memory: result[0] = 1 if some offs[i] > offs[i + 1] or offs[n_docs] > hay_len (left as it
+// was otherwise: the caller clears it), result[1] = offs[0], result[2] = offs[n_docs].
+cudaError_t launch_check_offsets(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
+                                 unsigned long long* result, cudaStream_t s);
+
 // K3/K3b: position-parallel k-gram prefilter fused with the anchored DFA verify.
 // Plays the role of the reference's packed/Teddy prefilter (src/packed/teddy/
 // generic.rs:114-713 candidate + :820-870 verify): a cheap per-position

@@ -8,6 +8,8 @@
 //                                 empty-pattern automata), one thread per document
 //        doc_flags_kernel         per-document is_match / first match of a batch's
 //        doc_first_kernel         prefilter tuples
+//        doc_records_kernel       device-resident batch records + their CSR index by document
+//        check_offsets_kernel     validation of document offsets in device memory
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
 #ifndef ACB_PTX_HEADER
@@ -350,6 +352,36 @@ __global__ void doc_first_kernel(DocFlagsLaunch f) {
   f.flags[doc] = 1;
 }
 
+// Ordered tuples of a batch -> acg_doc_match records and their CSR index by document, in one pass (see
+// DocRecordsLaunch).  No match crosses a document end, so the documents of the records do not decrease.
+__global__ void doc_records_kernel(DocRecordsLaunch e) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= e.n) return;
+  const uint32_t pid = e.pids[i];
+  const MatchSpan m = decode_key(e.keys[i], pid, e.mode, e.span_start, e.pattern_lens);
+  const uint64_t doc = doc_of(e.doc_offsets, e.n_docs, m.start);
+  const uint64_t base = e.doc_offsets[doc];
+  e.out[i * 3 + 0] = (uint64_t)pid | doc << 32;
+  e.out[i * 3 + 1] = m.start - base;
+  e.out[i * 3 + 2] = m.end - base;
+  uint64_t d = 0;
+  if (i) d = doc_of(e.doc_offsets, e.n_docs, decode_key(e.keys[i - 1], e.pids[i - 1], e.mode, e.span_start, e.pattern_lens).start) + 1;
+  for (; d <= doc; ++d) e.match_offsets[d] = i;
+  if (i + 1 == e.n)
+    for (d = doc + 1; d <= e.n_docs; ++d) e.match_offsets[d] = e.n;
+}
+
+__global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
+                                     unsigned long long* result) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) {
+    result[1] = offs[0];
+    result[2] = offs[n_docs];
+    if (offs[n_docs] > hay_len) result[0] = 1;
+  }
+  if (i < n_docs && offs[i] > offs[i + 1]) result[0] = 1;  // every writer stores the same word
+}
+
 // Records built in shared memory and stored as 16-byte vectors: the target may be another GPU's HBM
 // (peer mapping of rank 0's receive buffer, acb_comm.hpp), where full lines per warp store matter
 // more than at home.  Two sizes: 256 records per CTA, and a small one -- 128 threads, 3 KB of shared
@@ -452,6 +484,18 @@ cudaError_t launch_doc_first(const DocFlagsLaunch& f, cudaStream_t s) {
   if (f.n == 0) return cudaGetLastError();
   ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
   ACB_LAUNCH(doc_first_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_doc_records(const DocRecordsLaunch& e, cudaStream_t s) {
+  if (e.n == 0) return cudaSuccess;
+  ACB_LAUNCH(doc_records_kernel, (unsigned)((e.n + 255) / 256), 256, 0, s, e);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_check_offsets(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
+                                 unsigned long long* result, cudaStream_t s) {
+  ACB_LAUNCH(check_offsets_kernel, (unsigned)(n_docs / 256 + 1), 256, 0, s, offs, n_docs, hay_len, result);
   return cudaGetLastError();
 }
 

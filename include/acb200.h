@@ -231,6 +231,37 @@ int acg_find_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, ui
                    const uint64_t* doc_offsets, uint64_t n_docs, int anchored, int earliest,
                    acg_doc_match* out, uint8_t* found);
 
+/* Batched search with device-resident inputs and results.  d_hay: device pointer to byte 0.
+ * doc_offsets: [n_docs + 1] CSR bounds, in host memory (offsets_on_device == 0) or device memory
+ * (!= 0, 8-byte aligned); device offsets are used by the kernels where they are, without a copy.
+ * Same contract and error codes as the acg_*_batch calls above:
+ * - per document, the same records in the same order;
+ * - decreasing offsets or offsets past hay_len give ACG_E_INVALID_SPAN, detected on the device
+ *   when the offsets are there;
+ * - n_docs >= 2^32 gives ACG_E_INVALID_ARG.
+ * All outputs are device pointers.  The call returns once they are written.
+ * find_iter / overlapping: d_out[0 .. *n_out) holds the acg_doc_match records, in the order and
+ * layout acg_*_batch writes to host memory, and d_match_offsets[n_docs + 1] their CSR index by
+ * document: the records of document d are d_out[d_match_offsets[d] .. d_match_offsets[d + 1]).
+ * If *n_out > cap the call returns ACG_E_OVERFLOW with the required count in *n_out and writes
+ * neither array (two-call protocol).  n_out is a host pointer: the only result that crosses to the
+ * host.  is_match / find: d_flags / d_found and d_out have n_docs entries, as in acg_is_match_batch /
+ * acg_find_batch. */
+int acg_find_iter_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_len,
+                               const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                               int anchored, acg_doc_match* d_out, uint64_t cap,
+                               uint64_t* d_match_offsets, uint64_t* n_out);
+int acg_find_overlapping_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_len,
+                                      const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                                      int anchored, acg_doc_match* d_out, uint64_t cap,
+                                      uint64_t* d_match_offsets, uint64_t* n_out);
+int acg_is_match_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_len,
+                              const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                              int anchored, uint8_t* d_flags);
+int acg_find_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_len,
+                          const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                          int anchored, int earliest, acg_doc_match* d_out, uint8_t* d_found);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

@@ -2,7 +2,7 @@
 """Batched search over many documents in one device call (acg_find_overlapping_batch, acg_find_batch).
 
     python tools/bench_docs.py [--hay-gib 4] [--steps 20] [--warmup 5] [--engine 0]
-                               [--call overlapping|find] [--workload cfg2|cfg3]
+                               [--call overlapping|find] [--workload cfg2|cfg3] [--out host|device]
 
 cfg 2's automaton and haystack (same seeds as bench.py), device-resident, cut at seeded boundaries into
 documents of log-uniform length in [16 B, 16 KiB] (~1.8 M documents, mean ~2.4 KiB at 4 GiB).  Prints one
@@ -17,6 +17,11 @@ card's name and power limit, and two checks outside the timed region:
 or on cfg 3 (leftmost-first, case-insensitive, built as bench.py builds it: the leftmost reduction).  Its
 checks: find_batch equals the first find_iter_batch record of every document, and 10 000 single find
 calls against one find_batch call over the same documents (host haystack, same results).
+
+--out device times the device-output form of the call instead (find_overlapping_iter_batch_torch /
+find_batch_torch, acg_*_batch_devout): offsets a CUDA tensor, results left in device memory.  Its results are
+checked equal to the host-output call's, and the checks above then run as usual.  wall_ms_per_step (host
+clock around calls that end in a device synchronise) is the number to compare between --out host and device.
 """
 import argparse
 import importlib.util
@@ -57,19 +62,28 @@ def bench_find(args, ac, d_hay, offs, ClockSampler):
     import aho_corasick_b200 as ab
     n, n_docs = d_hay.numel(), offs.size - 1
     batch = (d_hay, offs)
+    call = ac.find_batch_np
+    if args.out == "device":
+        import torch
+        d_offs = torch.from_numpy(offs).cuda()
+        call = lambda _: ac.find_batch_torch((d_hay, d_offs))  # noqa: E731
     for _ in range(args.warmup):
-        found, rec = ac.find_batch_np(batch)
+        found, rec = call(batch)
     kernel_ms, scan_ms, order_ms = [], [], []
     with ClockSampler(0) as clocks:
         t0 = time.perf_counter()
         for _ in range(args.steps):
-            found, rec = ac.find_batch_np(batch)
+            found, rec = call(batch)
             st = ac.last_stats()
             kernel_ms.append(st["scan_ms"] + st["order_ms"])
             scan_ms.append(st["scan_ms"])
             order_ms.append(st["order_ms"])
         wall = time.perf_counter() - t0
     engine, tuples = int(st["engine"]), int(st["raw_matches"])
+    if args.out == "device":  # equal to the host-output call, then checked like it
+        d_found, d_rec = found.cpu().numpy(), rec.cpu().numpy()
+        found, rec = ac.find_batch_np(batch)
+        assert np.array_equal(d_found, found) and d_rec.tobytes() == rec.tobytes(), "device output differs"
     # check 1: the first find_iter_batch record of every document
     it = ac.find_iter_batch_np(batch)
     idx = np.flatnonzero(np.r_[True, it["doc"][1:] != it["doc"][:-1]]) if len(it) else np.zeros(0, np.int64)
@@ -103,6 +117,7 @@ def bench_find(args, ac, d_hay, offs, ClockSampler):
                     "[16 B, 16 KiB], the first match of every document (find) in one batch call",
         "haystack_bytes": n, "documents": n_docs, "mean_document_bytes": n / n_docs,
         "engine": {2: "prefilter_kernel + doc_first_kernel", 3: "seq_docs_kernel"}.get(engine, engine),
+        "out": args.out,
         "documents_with_a_match": int(found.sum()), "tuples_reduced": tuples,
         "scan_ms": sum(scan_ms) / len(scan_ms), "order_ms": sum(order_ms) / len(order_ms),
         "timing": "CUDA events inside the library: scan + per-document reduction of the batch call",
@@ -122,6 +137,8 @@ def main():
     ap.add_argument("--engine", type=int, default=0, help="0 auto, 3 the per-document sequential kernel")
     ap.add_argument("--call", default="overlapping", choices=["overlapping", "find"])
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg3"])
+    ap.add_argument("--out", default="host", choices=["host", "device"],
+                    help="results to host memory (acg_*_batch) or left in device memory (acg_*_batch_devout)")
     args = ap.parse_args()
     if args.call == "overlapping" and args.workload != "cfg2":
         ap.error("find_overlapping_iter needs cfg 2's Standard automaton")
@@ -145,19 +162,27 @@ def main():
     if args.call == "find":
         return bench_find(args, ac, d_hay, offs, ClockSampler)
     batch = (d_hay, offs)
+    call = ac.find_overlapping_iter_batch_np
+    if args.out == "device":
+        d_offs = torch.from_numpy(offs).cuda()
+        call = lambda _: ac.find_overlapping_iter_batch_torch((d_hay, d_offs))  # noqa: E731
     for _ in range(args.warmup):
-        got = ac.find_overlapping_iter_batch_np(batch)
+        got = call(batch)
     kernel_ms, scan_ms, order_ms = [], [], []
     with ClockSampler(0) as clocks:
         t0 = time.perf_counter()
         for _ in range(args.steps):
-            got = ac.find_overlapping_iter_batch_np(batch)
+            got = call(batch)
             st = ac.last_stats()
             kernel_ms.append(st["scan_ms"] + st["order_ms"])
             scan_ms.append(st["scan_ms"])
             order_ms.append(st["order_ms"])
         wall = time.perf_counter() - t0
     engine = int(ac.last_stats()["engine"])
+    if args.out == "device":  # equal to the host-output call, then checked like it
+        d_rec = got.records.cpu().numpy()
+        got = ac.find_overlapping_iter_batch_np(batch)
+        assert d_rec.tobytes() == got.tobytes(), "device output differs"
     ac.set_engine(ab.Engine.Auto)
     single, _ = ac.find_overlapping_iter_dev_np(d_hay.data_ptr(), n)
     doc = np.searchsorted(offs, single["start"].astype(np.int64), side="right") - 1
@@ -190,7 +215,7 @@ def main():
         "workload": "cfg2's automaton and haystack cut into documents of log-uniform length in [16 B, 16 KiB], "
                     "find_overlapping_iter of every document in one batch call",
         "haystack_bytes": n, "documents": int(offs.size - 1), "mean_document_bytes": n / (offs.size - 1),
-        "engine": {2: "prefilter_kernel", 3: "seq_docs_kernel"}.get(engine, engine),
+        "engine": {2: "prefilter_kernel", 3: "seq_docs_kernel"}.get(engine, engine), "out": args.out,
         "matches": len(got), "scan_ms": sum(scan_ms) / len(scan_ms), "order_ms": sum(order_ms) / len(order_ms),
         "timing": "CUDA events inside the library: scan + order of the batch call on the search stream",
         "wall_ms_per_step": wall / args.steps * 1e3,
