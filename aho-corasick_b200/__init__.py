@@ -494,6 +494,22 @@ class AhoCorasickBuilder:
         return AhoCorasick(h)
 
 
+def _until_it_fits(owner, cap, alloc, cnt, call):
+    """The caller's side of the two-call overflow protocol: `call(out, cap)` on `out = alloc(cap)`, again with
+    room to spare while it returns E_OVERFLOW (the call leaves the required count in `cnt`); `owner` keeps
+    the capacity that was needed as a hint for its next search.  Returns out[:count]."""
+    while True:
+        out = alloc(cap)
+        rc = call(out, cap)
+        if rc == E_OVERFLOW:
+            cap = int(cnt.value) + int(cnt.value) // 8 + 64
+            owner._cap_hint = max(owner._cap_hint, cap)
+            continue
+        if rc:
+            owner._raise(rc)
+        return out[: cnt.value]
+
+
 class AhoCorasick:
     """`AhoCorasick`, src/ahocorasick.rs:177-2082 (search surface only; replace/stream are out of scope)."""
 
@@ -636,18 +652,10 @@ class AhoCorasick:
         s, e = _span(span, n)
         # room for one match per 256 haystack bytes from the start (the device sizes its own tuple buffer the
         # same way): an overflow retry repeats the whole copy + scan, so it should be the exception
-        cap = max(self._cap_hint, max(e - s, 0) // 256 + 64)
-        while True:
-            out = np.empty(cap, MATCH_DTYPE)
-            cnt = _u64()
-            rc = fn(self._h, ptr, n, s, e, int(anchored), out.ctypes.data, cap, C.byref(cnt))
-            if rc == E_OVERFLOW:  # the call reports the required count: retry once with room to spare
-                cap = int(cnt.value) + int(cnt.value) // 8 + 64
-                self._cap_hint = max(self._cap_hint, cap)
-                continue
-            if rc:
-                self._raise(rc)
-            return out[: cnt.value]
+        cnt = _u64()
+        return _until_it_fits(
+            self, max(self._cap_hint, max(e - s, 0) // 256 + 64), lambda cap: np.empty(cap, MATCH_DTYPE), cnt,
+            lambda out, cap: fn(self._h, ptr, n, s, e, int(anchored), out.ctypes.data, cap, C.byref(cnt)))
 
     def try_find_iter_np(self, hay, span=None, anchored=Anchored.No):
         return self._collect(_lib.acg_find_iter, hay, span, anchored)
@@ -713,19 +721,12 @@ class AhoCorasick:
     def _collect_batch(self, fn, docs, anchored):
         keep, ptr, n, on_dev, offs = _batch_input(docs)
         n_docs = offs.size - 1
-        cap = max(self._cap_hint, n // 256 + 64)
-        while True:
-            out = np.empty(cap, DOC_MATCH_DTYPE)
-            cnt = _u64()
-            rc = fn(self._h, ptr, on_dev, n, offs.ctypes.data, n_docs, int(anchored), out.ctypes.data, cap,
-                    C.byref(cnt))
-            if rc == E_OVERFLOW:
-                cap = int(cnt.value) + int(cnt.value) // 8 + 64
-                self._cap_hint = max(self._cap_hint, cap)
-                continue
-            if rc:
-                self._raise(rc)
-            return out[: cnt.value], n_docs
+        cnt = _u64()
+        out = _until_it_fits(
+            self, max(self._cap_hint, n // 256 + 64), lambda cap: np.empty(cap, DOC_MATCH_DTYPE), cnt,
+            lambda out, cap: fn(self._h, ptr, on_dev, n, offs.ctypes.data, n_docs, int(anchored), out.ctypes.data,
+                                cap, C.byref(cnt)))
+        return out, n_docs
 
     @staticmethod
     def _per_doc(r, n_docs):
@@ -827,21 +828,12 @@ class AhoCorasick:
         import torch
         values, keep, optr, n_docs, on_dev = _torch_batch(docs)
         match_offsets = torch.empty(n_docs + 1, dtype=torch.int64, device=values.device)
-        cap = self._cap_hint
-        for _ in range(2):
-            records = torch.empty((cap, 3), dtype=torch.int64, device=values.device)
-            cnt = _u64()
-            rc = fn(self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs, int(anchored),
-                    records.data_ptr(), cap, match_offsets.data_ptr(), C.byref(cnt))
-            if rc == E_OVERFLOW:  # retry once with the reported count and room to spare
-                cap = int(cnt.value) + int(cnt.value) // 8 + 64
-                self._cap_hint = max(self._cap_hint, cap)
-                continue
-            if rc:
-                self._raise(rc)
-            r = records[: cnt.value]
-            return BatchMatches(r, match_offsets, r[:, 0] & 0xFFFFFFFF, r[:, 0] >> 32, r[:, 1], r[:, 2])
-        raise DeviceError(E_OVERFLOW)
+        cnt = _u64()
+        r = _until_it_fits(
+            self, self._cap_hint, lambda cap: torch.empty((cap, 3), dtype=torch.int64, device=values.device), cnt,
+            lambda records, cap: fn(self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs, int(anchored),
+                                    records.data_ptr(), cap, match_offsets.data_ptr(), C.byref(cnt)))
+        return BatchMatches(r, match_offsets, r[:, 0] & 0xFFFFFFFF, r[:, 0] >> 32, r[:, 1], r[:, 2])
 
     def find_iter_batch_torch(self, docs, anchored=Anchored.No):
         """find_iter of every document, results on the device: a BatchMatches of CUDA tensors."""
@@ -1006,35 +998,21 @@ class AhoCorasick:
     # ---- device-resident haystack (torch tensor / raw pointer), for the roofline measurement ----
     def find_overlapping_iter_dev_np(self, dev_ptr, hay_len, span=None):
         s, e = _span(span, hay_len)
-        cap = max(self._cap_hint, 1 << 16)
-        while True:
-            out = np.empty(cap, MATCH_DTYPE)
-            cnt, ms = _u64(), C.c_float()
-            rc = _lib.acg_find_overlapping_dev(self._h, dev_ptr, hay_len, s, e, out.ctypes.data, cap,
-                                               C.byref(cnt), C.byref(ms))
-            if rc == E_OVERFLOW:
-                cap = int(cnt.value) + int(cnt.value) // 8 + 64
-                self._cap_hint = max(self._cap_hint, cap)
-                continue
-            if rc:
-                self._raise(rc)
-            return out[: cnt.value], ms.value
+        cnt, ms = _u64(), C.c_float()
+        out = _until_it_fits(
+            self, max(self._cap_hint, 1 << 16), lambda cap: np.empty(cap, MATCH_DTYPE), cnt,
+            lambda out, cap: _lib.acg_find_overlapping_dev(self._h, dev_ptr, hay_len, s, e, out.ctypes.data, cap,
+                                                           C.byref(cnt), C.byref(ms)))
+        return out, ms.value
 
     def find_iter_dev_np(self, dev_ptr, hay_len, span=None):
         s, e = _span(span, hay_len)
-        cap = max(self._cap_hint, 1 << 16)
-        while True:
-            out = np.empty(cap, MATCH_DTYPE)
-            cnt, ms = _u64(), C.c_float()
-            rc = _lib.acg_find_iter_dev(self._h, dev_ptr, hay_len, s, e, out.ctypes.data, cap,
-                                        C.byref(cnt), C.byref(ms))
-            if rc == E_OVERFLOW:
-                cap = int(cnt.value) + int(cnt.value) // 8 + 64
-                self._cap_hint = max(self._cap_hint, cap)
-                continue
-            if rc:
-                self._raise(rc)
-            return out[: cnt.value], ms.value
+        cnt, ms = _u64(), C.c_float()
+        out = _until_it_fits(
+            self, max(self._cap_hint, 1 << 16), lambda cap: np.empty(cap, MATCH_DTYPE), cnt,
+            lambda out, cap: _lib.acg_find_iter_dev(self._h, dev_ptr, hay_len, s, e, out.ctypes.data, cap,
+                                                    C.byref(cnt), C.byref(ms)))
+        return out, ms.value
 
     def find_overlapping_devout(self, dev_ptr, hay_len, span, min_end, offset_add, out_ptr, cap):
         """Ordered matches stay on the device (acg_match records at out_ptr). Returns (n, kernel_ms);

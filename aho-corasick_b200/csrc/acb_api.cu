@@ -41,37 +41,72 @@ namespace {
 // [kBucketCountersAt + b] the tuples of bucket b
 constexpr size_t kCounterBytes = 8 * (acb::kBucketCountersAt + acb::kMaxBuckets);
 
+// A buffer that owns its memory -- device, or page-locked host -- and only grows.  A grow discards the
+// contents; after a failed allocation the buffer is empty, so a capacity never outlives its memory.
+template <class T, bool kPinned>
+struct Buf {
+  T* p = nullptr;
+  uint64_t cap = 0;  // elements
+  Buf() = default;
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  ~Buf() { release(); }
+  operator T*() const { return p; }
+  void release() {
+    if (p) kPinned ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    cap = 0;
+  }
+  int reserve(uint64_t n) {
+    if (n <= cap) return ACG_OK;
+    release();
+    const cudaError_t e = kPinned ? cudaMallocHost(&p, n * sizeof(T)) : cudaMalloc(&p, n * sizeof(T));
+    if (e != cudaSuccess) p = nullptr;
+    CK(e);
+    cap = n;
+    return ACG_OK;
+  }
+};
+template <class T> using DevBuf = Buf<T, false>;
+template <class T> using PinnedBuf = Buf<T, true>;
+
+// Room for n elements in each of several buffers that share a sizing policy, or none of them: the ones that
+// are too small are all released before the first is allocated (a grow never holds the old and the new memory
+// together), and when an allocation fails the whole group is released, so that the next search starts from
+// nothing instead of from a capacity that only some of the group have.
+template <class... B>
+int reserve_all(uint64_t n, B&... b) {
+  ((b.cap < n ? b.release() : void()), ...);
+  int rc = ACG_OK;
+  ((rc = rc ? rc : b.reserve(n)), ...);
+  if (rc) (b.release(), ...);
+  return rc;
+}
+
 struct Workspace {
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
-  uint64_t cap = 0;  // tuple capacity
-  uint64_t* d_keys[2] = {nullptr, nullptr};
-  uint32_t* d_pids[2] = {nullptr, nullptr};
-  unsigned long long* d_counter = nullptr;
-  unsigned long long* h_counter = nullptr;  // pinned
-  void* d_temp = nullptr;  // CUB temporary storage (cub_call): a search's CUB calls run in order on `stream`
-  size_t temp_bytes = 0;
-  uint64_t* h_keys = nullptr;  // pinned staging
-  uint32_t* h_pids = nullptr;
-  uint64_t h_cap = 0;
-  uint8_t* d_hay = nullptr;  // staging of host haystacks
-  uint64_t d_hay_cap = 0;
-  uint64_t* d_scratch = nullptr;  // chain resolution: end offsets / prefix max [cap]
-  uint8_t* d_flags = nullptr;     // [cap]
-  uint64_t chain_cap = 0;
-  uint64_t* d_seq = nullptr;  // sequential engine output [cap*3]
-  uint64_t seq_cap = 0;
-  uint64_t* h_seq = nullptr;
-  uint64_t h_seq_cap = 0;
+  DevBuf<uint64_t> d_keys[2];  // the tuple lists: all four of one capacity, or all empty (reserve_tuples)
+  DevBuf<uint32_t> d_pids[2];
+  uint64_t tuple_cap() const { return d_keys[0].cap; }
+  DevBuf<unsigned long long> d_counter;
+  PinnedBuf<unsigned long long> h_counter;
+  DevBuf<uint8_t> d_temp;  // CUB temporary storage (cub_call): a search's CUB calls run in order on `stream`
+  PinnedBuf<uint64_t> h_keys;  // staging of the tuples on their way to the caller
+  PinnedBuf<uint32_t> h_pids;
+  DevBuf<uint8_t> d_hay;  // staging of host haystacks
+  DevBuf<uint64_t> d_scratch;  // chain resolution: end offsets / prefix max
+  DevBuf<uint8_t> d_flags;
+  DevBuf<uint64_t> d_seq;  // sequential engine output, three words per record
+  PinnedBuf<uint64_t> h_seq;
   acg_stats stats{};  // of the search that holds (or last held) this workspace
   // pageable host haystacks: page-locked staging ring filled by host threads (run_prefilter)
-  uint8_t* h_stage[2] = {nullptr, nullptr};
-  uint64_t h_stage_cap = 0;
+  PinnedBuf<uint8_t> h_stage[2];
   cudaEvent_t stage_ev[2] = {nullptr, nullptr};
-  // batched search: document offsets, per-document counts and their inclusive scan [3][docs_cap], flags [docs_cap]
-  uint64_t* d_docs = nullptr;
-  uint8_t* d_doc_flags = nullptr;
-  uint64_t docs_cap = 0;
+  // batched search, per document: offsets, counts, their inclusive scan, flags
+  DevBuf<uint64_t> d_doc_offs;
+  DevBuf<unsigned long long> d_doc_counts, d_doc_incl;
+  DevBuf<uint8_t> d_doc_flags;
 };
 
 }  // namespace
@@ -149,25 +184,15 @@ int init_workspace(Workspace& w) {
   CK(cudaEventCreate(&w.ev1));
   CK(cudaEventCreate(&w.ev2));
   CK(cudaEventCreate(&w.ev3));
-  CK(cudaMalloc(&w.d_counter, kCounterBytes));
-  CK(cudaMallocHost(&w.h_counter, kCounterBytes));
-  return ACG_OK;
+  int rc = w.d_counter.reserve(kCounterBytes / 8);
+  return rc ? rc : w.h_counter.reserve(kCounterBytes / 8);
 }
 
+// The buffers free themselves when the workspace is deleted: right after this, on the handle's device.
 void destroy_workspace(Workspace& w) {
   if (w.stream) cudaStreamSynchronize(w.stream);
-  for (int i = 0; i < 2; ++i) { cudaFree(w.d_keys[i]); cudaFree(w.d_pids[i]); }
-  cudaFree(w.d_counter); cudaFree(w.d_temp); cudaFree(w.d_hay); cudaFree(w.d_seq);
-  cudaFree(w.d_scratch); cudaFree(w.d_flags);
-  cudaFree(w.d_docs); cudaFree(w.d_doc_flags);
-  if (w.h_counter) cudaFreeHost(w.h_counter);
-  if (w.h_keys) cudaFreeHost(w.h_keys);
-  if (w.h_pids) cudaFreeHost(w.h_pids);
-  if (w.h_seq) cudaFreeHost(w.h_seq);
-  for (int i = 0; i < 2; ++i) {
-    if (w.h_stage[i]) cudaFreeHost(w.h_stage[i]);
+  for (int i = 0; i < 2; ++i)
     if (w.stage_ev[i]) cudaEventDestroy(w.stage_ev[i]);
-  }
   if (w.ev0) cudaEventDestroy(w.ev0);
   if (w.ev1) cudaEventDestroy(w.ev1);
   if (w.ev2) cudaEventDestroy(w.ev2);
@@ -714,21 +739,8 @@ int upload(acg_dfa* a) {
   return ACG_OK;
 }
 
-int ensure_tuple_cap(Workspace& w, uint64_t cap) {
-  if (cap <= w.cap) return ACG_OK;
-  for (int i = 0; i < 2; ++i) {
-    if (w.d_keys[i]) cudaFree(w.d_keys[i]);
-    if (w.d_pids[i]) cudaFree(w.d_pids[i]);
-    w.d_keys[i] = nullptr;
-    w.d_pids[i] = nullptr;
-  }
-  w.cap = 0;
-  for (int i = 0; i < 2; ++i) {
-    CK(cudaMalloc(&w.d_keys[i], cap * 8));
-    CK(cudaMalloc(&w.d_pids[i], cap * 4));
-  }
-  w.cap = cap;
-  return ACG_OK;
+int reserve_tuples(Workspace& w, uint64_t cap) {
+  return reserve_all(cap, w.d_keys[0], w.d_pids[0], w.d_keys[1], w.d_pids[1]);
 }
 
 // One CUB call `f(d_temp, temp_bytes)` on the workspace's temporary storage: sized by a query
@@ -737,74 +749,22 @@ template <class F>
 int cub_call(Workspace& w, F f) {
   size_t tb = 0;
   CK(f(nullptr, tb));
-  if (!w.d_temp || tb > w.temp_bytes) {
-    cudaFree(w.d_temp);
-    w.d_temp = nullptr;
-    w.temp_bytes = 0;
-    CK(cudaMalloc(&w.d_temp, std::max<size_t>(tb, 16)));
-    w.temp_bytes = std::max<size_t>(tb, 16);
-  }
-  tb = w.temp_bytes;
+  int rc = w.d_temp.reserve(std::max<size_t>(tb, 16));
+  if (rc) return rc;
+  tb = w.d_temp.cap;
   CK(f(w.d_temp, tb));
   return ACG_OK;
 }
 
-int ensure_host_staging(Workspace& w, uint64_t n) {
-  if (n <= w.h_cap) return ACG_OK;
-  if (w.h_keys) cudaFreeHost(w.h_keys);
-  if (w.h_pids) cudaFreeHost(w.h_pids);
-  w.h_keys = nullptr;
-  w.h_pids = nullptr;
-  w.h_cap = 0;
-  const uint64_t cap = std::max<uint64_t>(n, 1 << 16);
-  CK(cudaMallocHost(&w.h_keys, cap * 8));
-  CK(cudaMallocHost(&w.h_pids, cap * 4));
-  w.h_cap = cap;
-  return ACG_OK;
-}
-
-int ensure_hay(Workspace& w, uint64_t bytes) {
-  if (bytes <= w.d_hay_cap) return ACG_OK;
-  if (w.d_hay) cudaFree(w.d_hay);
-  w.d_hay = nullptr;
-  w.d_hay_cap = 0;
-  const uint64_t cap = ((bytes + (1ull << 20)) >> 20) << 20;
-  CK(cudaMalloc(&w.d_hay, cap));
-  w.d_hay_cap = cap;
-  return ACG_OK;
-}
-
-int ensure_seq(Workspace& w, uint64_t cap) {
-  if (cap > w.seq_cap) {
-    if (w.d_seq) cudaFree(w.d_seq);
-    w.d_seq = nullptr;
-    w.seq_cap = 0;
-    CK(cudaMalloc(&w.d_seq, cap * 24));
-    w.seq_cap = cap;
-  }
-  if (cap > w.h_seq_cap) {
-    if (w.h_seq) cudaFreeHost(w.h_seq);
-    w.h_seq = nullptr;
-    w.h_seq_cap = 0;
-    CK(cudaMallocHost(&w.h_seq, cap * 24));
-    w.h_seq_cap = cap;
-  }
-  return ACG_OK;
+// sequential engine, batched find: room for `cap` records on the device and on their way to the caller
+int reserve_seq(Workspace& w, uint64_t cap) {
+  int rc = w.d_seq.reserve(cap * 3);
+  return rc ? rc : w.h_seq.reserve(cap * 3);
 }
 
 // batched search: room for n entries in each per-document array
-int ensure_docs(Workspace& w, uint64_t n) {
-  if (n <= w.docs_cap) return ACG_OK;
-  cudaFree(w.d_docs);
-  cudaFree(w.d_doc_flags);
-  w.d_docs = nullptr;
-  w.d_doc_flags = nullptr;
-  w.docs_cap = 0;
-  const uint64_t cap = std::max<uint64_t>(n, 1 << 12);
-  CK(cudaMalloc(&w.d_docs, cap * 3 * 8));
-  CK(cudaMalloc(&w.d_doc_flags, cap));
-  w.docs_cap = cap;
-  return ACG_OK;
+int reserve_docs(Workspace& w, uint64_t n) {
+  return reserve_all(std::max<uint64_t>(n, 1 << 12), w.d_doc_offs, w.d_doc_counts, w.d_doc_incl, w.d_doc_flags);
 }
 
 // enforce_anchored_consistency, src/ahocorasick.rs:2778-2789
@@ -922,7 +882,7 @@ int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t rea
   p.keys = w.d_keys[0];
   p.pids = w.d_pids[0];
   p.counter = w.d_counter;
-  p.cap = w.cap;
+  p.cap = w.tuple_cap();
   p.bucket_shift = bp.shift;
   p.bucket_log = bp.log;
   p.bucket_slots = bp.slots();
@@ -1018,9 +978,9 @@ int run_walk_overlapping(const acg_dfa* a, const uint8_t* d_hay, uint64_t readab
   // shard starts are placed so that (d_hay + span_start + k*seg_len) keeps the 16-byte
   // phase of the first shard; the kernel handles the unaligned head per lane.
   const uint64_t n_segs = std::max<uint64_t>((n_bytes + seg_len - 1) / seg_len, 1);
-  uint64_t cap = std::max<uint64_t>(w.cap, std::max<uint64_t>(1 << 20, n_bytes / 256));
+  uint64_t cap = std::max<uint64_t>(w.tuple_cap(), std::max<uint64_t>(1 << 20, n_bytes / 256));
   for (int attempt = 0; attempt < 8; ++attempt) {
-    int rc = ensure_tuple_cap(w, cap);
+    int rc = reserve_tuples(w, cap);
     if (rc) return rc;
     CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
     acb::WalkLaunch p;
@@ -1033,7 +993,7 @@ int run_walk_overlapping(const acg_dfa* a, const uint8_t* d_hay, uint64_t readab
     p.keys = w.d_keys[0];
     p.pids = w.d_pids[0];
     p.counter = w.d_counter;
-    p.cap = w.cap;
+    p.cap = w.tuple_cap();
     CK(cudaEventRecord(w.ev0, w.stream));
     CK(acb::launch_walk_overlapping(a->dev, p, w.stream));
     CK(cudaEventRecord(w.ev1, w.stream));
@@ -1041,7 +1001,7 @@ int run_walk_overlapping(const acg_dfa* a, const uint8_t* d_hay, uint64_t readab
     CK(cudaStreamSynchronize(w.stream));
     cur_ws().stats.launches += 1;
     const uint64_t want = *w.h_counter;
-    if (want > w.cap) { cap = want + want / 8 + 1024; continue; }  // overflow: grow and rescan
+    if (want > w.tuple_cap()) { cap = want + want / 8 + 1024; continue; }  // overflow: grow and rescan
     float ms = 0;
     cudaEventElapsedTime(&ms, w.ev0, w.ev1);
     cur_ws().stats.scan_ms = ms;
@@ -1137,14 +1097,13 @@ bool is_pageable_host(const void* p) {
   return attr.type == cudaMemoryTypeUnregistered;
 }
 
-int ensure_stage(Workspace& w, uint64_t bytes) {
-  if (bytes <= w.h_stage_cap) return ACG_OK;
+// The staging ring of a pageable host haystack: two buffers of `bytes`, and the event that guards each.
+int reserve_stage(Workspace& w, uint64_t bytes) {
   for (int i = 0; i < 2; ++i) {
-    if (w.h_stage[i]) { cudaFreeHost(w.h_stage[i]); w.h_stage[i] = nullptr; }
-    CK(cudaMallocHost(&w.h_stage[i], bytes));
+    int rc = w.h_stage[i].reserve(bytes);
+    if (rc) return rc;
     if (!w.stage_ev[i]) CK(cudaEventCreateWithFlags(&w.stage_ev[i], cudaEventDisableTiming));
   }
-  w.h_stage_cap = bytes;
   return ACG_OK;
 }
 
@@ -1165,14 +1124,14 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
   cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, a->device);
   // one tuple per 256 haystack bytes to start with (the BASELINE workloads have one per 4 KiB);
   // denser outputs are detected through the counter and the scan is repeated with room
-  uint64_t cap = std::max<uint64_t>(w.cap, std::max<uint64_t>(1 << 20, (scan_hi - scan_lo) / 256));
+  uint64_t cap = std::max<uint64_t>(w.tuple_cap(), std::max<uint64_t>(1 << 20, (scan_hi - scan_lo) / 256));
   // bucketed emission: the buckets' slots, then at least 64 K slots of overflow list
   const BucketPlan bp = unordered ? BucketPlan{} : plan_buckets(a, n_bytes);
   cap = std::max<uint64_t>(cap, bp.slots() + (bp.shift ? (1u << 16) : 0));
   const size_t counter_bytes = bp.shift ? 8 * (acb::kBucketCountersAt + size_t(bp.n)) : 16;
   bool copied = h_hay == nullptr;
   for (int attempt = 0; attempt < 8; ++attempt) {
-    int rc = ensure_tuple_cap(w, cap);
+    int rc = reserve_tuples(w, cap);
     if (rc) return rc;
     CK(cudaMemsetAsync(w.d_counter, 0, counter_bytes, w.stream));
     CK(cudaEventRecord(w.ev0, w.stream));
@@ -1188,7 +1147,7 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
       uint64_t scanned = span_start;
       // pageable source: the chunk goes through a page-locked ring buffer filled by host threads
       const bool staged = span_end - span_start >= std::min<uint64_t>(8u << 20, chunk) && is_pageable_host(h_hay + span_start);
-      if (staged && (rc = ensure_stage(w, std::min<uint64_t>(chunk, span_end - span_start)))) return rc;
+      if (staged && (rc = reserve_stage(w, std::min<uint64_t>(chunk, span_end - span_start)))) return rc;
       bool stage_used[2] = {false, false};
       int stage_i = 0;
       CK(cudaEventRecord(w.ev2, w.copy_stream));
@@ -1224,12 +1183,12 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
     CK(cudaStreamSynchronize(w.stream));
     // bucketed: counter[0] is the length of the overflow list, the buckets' counters include the tuples
     // that went there
-    uint64_t want = w.h_counter[0], overflow = 0, room = w.cap;
+    uint64_t want = w.h_counter[0], overflow = 0, room = w.tuple_cap();
     if (bp.shift) {
       overflow = want;
       want = 0;
       for (uint32_t i = 0; i < bp.n; ++i) want += w.h_counter[acb::kBucketCountersAt + i];
-      room = w.cap - bp.slots();
+      room = w.tuple_cap() - bp.slots();
     }
     cur_ws().stats.candidates = w.h_counter[1];
     // the reference retires a prefilter that keeps reporting candidates (PrefilterState,
@@ -1240,9 +1199,9 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
     float ms = 0;
     cudaEventElapsedTime(&ms, w.ev0, w.ev1);
     cur_ws().stats.scan_ms = ms;  // with a host haystack this is the overlapped copy+scan time
-    if (bp.shift ? overflow > room : want > w.cap) {
+    if (bp.shift ? overflow > room : want > w.tuple_cap()) {
       const uint64_t need = bp.shift ? overflow : want;
-      cap = (w.cap - room) + need + need / 8 + 1024;
+      cap = (w.tuple_cap() - room) + need + need / 8 + 1024;
       continue;
     }
     if (unordered) {  // one list in buffer 0, in emission order
@@ -1256,16 +1215,9 @@ int run_prefilter(const acg_dfa* a, const uint8_t* d_hay, uint64_t readable, uin
   return ACG_E_NOMEM;
 }
 
-int ensure_chain(Workspace& w, uint64_t n) {
-  if (n <= w.chain_cap) return ACG_OK;
-  if (w.d_scratch) cudaFree(w.d_scratch);
-  if (w.d_flags) cudaFree(w.d_flags);
-  w.d_scratch = nullptr; w.d_flags = nullptr; w.chain_cap = 0;
-  const uint64_t cap = std::max<uint64_t>(n, 1 << 16);
-  CK(cudaMalloc(&w.d_scratch, cap * 8));
-  CK(cudaMalloc(&w.d_flags, cap));
-  w.chain_cap = cap;
-  return ACG_OK;
+// The ordered tuples of `r` as the kernels that read them take them.
+acb::TupleList tuple_list(const acg_dfa* a, const Workspace& w, const TupleResult& r) {
+  return acb::TupleList{w.d_keys[r.sorted_buf], w.d_pids[r.sorted_buf], a->d_plens, r.n};
 }
 
 // FindIter over ordered candidate tuples, on the device: marks the tuples the reference's
@@ -1273,14 +1225,11 @@ int ensure_chain(Workspace& w, uint64_t n) {
 int run_chain(const acg_dfa* a, int mode, TupleResult* r) {
   Workspace& w = cur_ws();
   if (r->n == 0) return ACG_OK;
-  int rc = ensure_chain(w, r->n);
+  int rc = reserve_all(std::max<uint64_t>(r->n, 1 << 16), w.d_scratch, w.d_flags);
   if (rc) return rc;
-  const int src = r->sorted_buf, dst = 1 - src;
+  const int dst = 1 - r->sorted_buf;
   acb::ChainLaunch c;
-  c.keys = w.d_keys[src];
-  c.pids = w.d_pids[src];
-  c.pattern_lens = a->d_plens;
-  c.n = r->n;
+  c.t = tuple_list(a, w, *r);
   c.mode = mode;
   c.scratch_end = w.d_scratch;
   c.flags = w.d_flags;
@@ -1291,8 +1240,8 @@ int run_chain(const acg_dfa* a, int mode, TupleResult* r) {
     return rc;
   CK(acb::launch_chain_select(c, w.stream));
   if ((rc = cub_call(w, [&](void* t, size_t& tb) {
-         return acb::select_flagged(t, tb, w.d_keys[src], w.d_pids[src], w.d_flags, w.d_keys[dst], w.d_pids[dst],
-                                    w.d_counter, r->n, w.stream);
+         return acb::select_flagged(t, tb, c.t.keys, c.t.pids, w.d_flags, w.d_keys[dst], w.d_pids[dst], w.d_counter,
+                                    r->n, w.stream);
        })))
     return rc;
   CK(cudaEventRecord(w.ev3, w.stream));
@@ -1318,11 +1267,12 @@ int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, ac
   if (fnv) *fnv = 0xcbf29ce484222325ull;
   if (r.n == 0) return ACG_OK;
   if (!fnv && r.n > cap) return ACG_E_OVERFLOW;
-  int rc = ensure_host_staging(w, r.n);
+  int rc = reserve_all(std::max<uint64_t>(r.n, 1 << 16), w.h_keys, w.h_pids);
   if (rc) return rc;
+  const acb::TupleList t = tuple_list(a, w, r);
   CK(cudaEventRecord(w.ev0, w.stream));
-  CK(cudaMemcpyAsync(w.h_keys, w.d_keys[r.sorted_buf], r.n * 8, cudaMemcpyDeviceToHost, w.stream));
-  CK(cudaMemcpyAsync(w.h_pids, w.d_pids[r.sorted_buf], r.n * 4, cudaMemcpyDeviceToHost, w.stream));
+  CK(cudaMemcpyAsync(w.h_keys, t.keys, r.n * 8, cudaMemcpyDeviceToHost, w.stream));
+  CK(cudaMemcpyAsync(w.h_pids, t.pids, r.n * 4, cudaMemcpyDeviceToHost, w.stream));
   CK(cudaEventRecord(w.ev1, w.stream));
   CK(cudaStreamSynchronize(w.stream));
   float ms = 0;
@@ -1361,16 +1311,16 @@ int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, ac
 int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_t span_end,
             int anchored, int earliest, int single, acg_match* out, uint64_t cap, uint64_t* n_out) {
   Workspace& w = cur_ws();
-  uint64_t scap = std::max<uint64_t>(std::max<uint64_t>(cap, 1024), w.seq_cap);
-  int rc = ensure_docs(w, 2);
+  uint64_t scap = std::max<uint64_t>(std::max<uint64_t>(cap, 1024), w.d_seq.cap / 3);
+  int rc = reserve_docs(w, 2);
   if (rc) return rc;
   const uint64_t bounds[2] = {span_start, span_end};
-  CK(cudaMemcpyAsync(w.d_docs, bounds, sizeof(bounds), cudaMemcpyHostToDevice, w.stream));
+  CK(cudaMemcpyAsync(w.d_doc_offs, bounds, sizeof(bounds), cudaMemcpyHostToDevice, w.stream));
   for (int attempt = 0; attempt < 4; ++attempt) {
-    if ((rc = ensure_seq(w, scap))) return rc;
+    if ((rc = reserve_seq(w, scap))) return rc;
     acb::SeqDocsLaunch p{};
     p.hay = d_hay;
-    p.doc_offsets = w.d_docs;
+    p.doc_offsets = w.d_doc_offs;
     p.n_docs = 1;
     p.anchored = anchored;
     p.match_kind = a->h.match_kind;
@@ -1378,7 +1328,7 @@ int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_
     p.single = single;
     p.counts = w.d_counter;
     p.out = w.d_seq;
-    p.cap = w.seq_cap;
+    p.cap = w.d_seq.cap / 3;
     CK(cudaEventRecord(w.ev0, w.stream));
     CK(acb::launch_seq_docs(a->dev, p, w.stream));
     CK(cudaEventRecord(w.ev1, w.stream));
@@ -1392,7 +1342,7 @@ int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_
     *n_out = n;
     cur_ws().stats.raw_matches = n;
     if (n > cap) return ACG_E_OVERFLOW;  // caller retries with a bigger buffer (two-call protocol)
-    if (n > w.seq_cap) { scap = n; continue; }
+    if (n > w.d_seq.cap / 3) { scap = n; continue; }
     if (n) {
       CK(cudaMemcpyAsync(w.h_seq, w.d_seq, n * 24, cudaMemcpyDeviceToHost, w.stream));
       CK(cudaStreamSynchronize(w.stream));
@@ -1416,8 +1366,11 @@ int stage_host_span(const acg_dfa* a, const uint8_t* hay, uint64_t span_start, u
   // keep the 16-byte phase of the host offsets so vector loads stay aligned
   const uint64_t lead = span_start & 15;
   const uint64_t bytes = span_end - span_start;
-  int rc = ensure_hay(w, bytes + lead + 64);
-  if (rc) return rc;
+  const uint64_t need = bytes + lead + 64;
+  if (need > w.d_hay.cap) {  // whole MiB, one past what is needed
+    int rc = w.d_hay.reserve(((need + (1ull << 20)) >> 20) << 20);
+    if (rc) return rc;
+  }
   *d_base = w.d_hay + lead - span_start;  // never dereferenced outside [span_start, span_end + slack)
   if (alloc_only) return ACG_OK;
   CK(cudaEventRecord(w.ev0, w.stream));
@@ -1515,7 +1468,7 @@ int scan_overlapping(const acg_dfa* a, const uint8_t* hay, bool on_device, uint6
   else rc = run_walk_overlapping(a, pl.base, pl.readable, span_start, span_end, r);
   if (rc || r->n == 0 || min_end <= span_start) return rc;
   const uint64_t bound_key = (min_end - span_start + 1) << acb::kTieBits;  // first key with end > min_end
-  CK(acb::launch_lower_bound(w.d_keys[r->sorted_buf], r->n, bound_key, w.d_counter, w.stream));
+  CK(acb::launch_lower_bound(tuple_list(a, w, *r).keys, r->n, bound_key, w.d_counter, w.stream));
   CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 8, cudaMemcpyDeviceToHost, w.stream));
   CK(cudaStreamSynchronize(w.stream));
   *first = *w.h_counter;
@@ -1553,10 +1506,7 @@ int overlapping_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, u
     *n_out = kept;
     if (kept > cap) return ACG_E_OVERFLOW;
     acb::ExpandLaunch e;
-    e.keys = w.d_keys[r.sorted_buf];
-    e.pids = w.d_pids[r.sorted_buf];
-    e.pattern_lens = a->d_plens;
-    e.n = r.n;
+    e.t = tuple_list(a, w, r);
     e.first = first;
     e.span_start = span_start;
     e.offset_add = devout->offset_add;
@@ -1643,10 +1593,7 @@ int sharded_begin(const acg_dfa* a, acg_comm* c, const uint8_t* hay, bool hay_on
   if (mine) {
     Workspace& w = cur_ws();
     acb::ExpandLaunch e;
-    e.keys = w.d_keys[r.sorted_buf];
-    e.pids = w.d_pids[r.sorted_buf];
-    e.pattern_lens = a->d_plens;
-    e.n = r.n;
+    e.t = tuple_list(a, w, r);
     e.first = first;
     e.span_start = lspan_s;
     e.offset_add = hay_off;
@@ -1755,6 +1702,89 @@ int find_iter_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uin
   return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, mode);
 }
 
+// acg_find (include/acb200.h)
+int find_impl(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,
+              uint64_t span_end, int anchored, int earliest, acg_match* out, int* found) {
+  if (!out || !found) return ACG_E_INVALID_ARG;
+  *found = 0;
+  int rc = validate_common(a, hay_len, span_start, span_end, anchored);
+  if (rc) return rc;
+  if ((rc = check_start(a->h, anchored))) return rc;
+  if (!a->on_device) return ACG_E_NO_DEVICE;
+  if (span_start > span_end) return ACG_OK;
+  earliest = find_earliest(a, anchored, earliest);
+  DeviceGuard guard(a->device);
+  WsLease lease(a);
+  if (lease.rc) return lease.rc;
+  Workspace& w = cur_ws();
+  const int engine = choose_engine(a, anchored, earliest, ACG_ENGINE_SEQUENTIAL, false);
+  w.stats.engine = engine;
+  // the prefilter engine's window-by-window copy below only takes the room
+  Placement pl;
+  if ((rc = place_input(a, hay, false, hay_len, span_start, span_end, engine == ACG_ENGINE_PREFILTER, &pl))) return rc;
+  if (engine == ACG_ENGINE_SEQUENTIAL) {
+    uint64_t n = 0;
+    rc = run_seq(a, pl.base, span_start, span_end, anchored, earliest, 1, out, 1, &n);
+    if (rc == ACG_OK && n) *found = 1;
+    return rc;
+  }
+  // The reference's try_find is lazy (it stops reading at the first match, SURVEY.md section
+  // 7h); the eager device scan therefore works through geometrically growing windows of start
+  // offsets (1 MiB, 16 MiB, 256 MiB, ...), copying only what a window needs.
+  const int mode = a->h.match_kind == ACG_STANDARD ? 0 : 1;
+  const uint64_t look = a->h.max_pattern_len + 64;
+  uint64_t copied_hi = span_start;
+  // Scan the start offsets [lo, hi) and fetch the first tuple (*n: the number of tuples).
+  auto first_in = [&](uint64_t lo, uint64_t hi, uint64_t* key, uint32_t* pid, uint64_t* n) -> int {
+    const uint64_t upto = std::min(hi + look, span_end);
+    if (upto > copied_hi) {
+      CK(cudaMemcpyAsync(const_cast<uint8_t*>(pl.base) + copied_hi, hay + copied_hi, upto - copied_hi,
+                         cudaMemcpyHostToDevice, w.stream));
+      copied_hi = upto;
+    }
+    TupleResult r;
+    int rc = run_prefilter(a, pl.base, copied_hi == span_end ? span_end + 32 : copied_hi, span_start, span_end,
+                           mode == 0 ? 2 : 1, &r, nullptr, lo, hi);
+    *n = r.n;
+    if (rc || r.n == 0) return rc;
+    const acb::TupleList t = tuple_list(a, w, r);
+    CK(cudaMemcpyAsync(w.h_counter, t.keys, 8, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaMemcpyAsync(w.h_counter + 1, t.pids, 4, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    *key = w.h_counter[0];
+    *pid = uint32_t(w.h_counter[1]);
+    return ACG_OK;
+  };
+  const uint32_t* plens = a->h.pattern_lens.data();
+  uint64_t lo = span_start, win = 1ull << 20;
+  while (lo < span_end) {
+    const uint64_t hi = std::min(span_end, lo + win);
+    uint64_t key = 0, n = 0;
+    uint32_t pid = 0;
+    if ((rc = first_in(lo, hi, &key, &pid, &n))) return rc;
+    if (n) {
+      const uint64_t end = acb::decode_key(key, pid, mode, span_start, plens).end;
+      if (mode == 0 && end > hi && hi < span_end) {
+        // Standard: a match that starts in [hi, end) could still end earlier -- scan those starts
+        uint64_t key2 = 0, n2 = 0;
+        uint32_t pid2 = 0;
+        if ((rc = first_in(hi, std::min(span_end, end), &key2, &pid2, &n2))) return rc;
+        if (n2 && key2 < key) { key = key2; pid = pid2; }
+      }
+      const acb::MatchSpan m = acb::decode_key(key, pid, mode, span_start, plens);
+      out->pid = pid;
+      out->_pad = 0;
+      out->start = m.start;
+      out->end = m.end;
+      *found = 1;
+      return ACG_OK;
+    }
+    lo = hi;
+    win = std::min<uint64_t>(win * 16, 1ull << 30);
+  }
+  return ACG_OK;
+}
+
 enum BatchKind { kBatchFindIter = 0, kBatchOverlapping = 1, kBatchIsMatch = 2, kBatchFind = 3 };
 
 // acg_*_batch_devout: the results stay in device memory -- `out` / `flags` are device pointers, and find_iter /
@@ -1802,12 +1832,12 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   Workspace& w = cur_ws();
   w.stats.engine = engine;
   const uint64_t nd1 = n_docs + 1;
-  if ((rc = ensure_docs(w, nd1))) return rc;
-  if (what == kBatchFind && !dv && (rc = ensure_seq(w, n_docs))) return rc;  // the records, at index doc
+  if ((rc = reserve_docs(w, nd1))) return rc;
+  if (what == kBatchFind && !dv && (rc = reserve_seq(w, n_docs))) return rc;  // the records, at index doc
   uint64_t span_start, span_end;
-  const uint64_t* d_offs = w.d_docs;
-  unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(w.d_docs + w.docs_cap);
-  unsigned long long* d_incl = d_counts + w.docs_cap;
+  const uint64_t* d_offs = w.d_doc_offs;
+  unsigned long long* const d_counts = w.d_doc_counts;
+  unsigned long long* const d_incl = w.d_doc_incl;
   if (offs_on_device) {
     // checked where they are; the span bounds come back with the verdict (placement and the scan plan need them)
     CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
@@ -1822,7 +1852,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   } else {
     span_start = offs[0];
     span_end = offs[n_docs];
-    CK(cudaMemcpyAsync(w.d_docs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
+    CK(cudaMemcpyAsync(w.d_doc_offs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
   }
   if (n_docs == 0) {  // device output: the index of no records
     if (!per_doc) CK(cudaMemsetAsync(dv->match_offsets, 0, 8, w.stream));
@@ -1833,7 +1863,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if ((rc = place_input(a, hay, hay_on_device, hay_len, span_start, span_end, use_pf, &pl))) return rc;
   // per-document results: the caller's device arrays, or the workspace's and a copy to the host
   uint8_t* d_flags = dv ? flags : w.d_doc_flags;
-  uint64_t* d_find = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq;
+  uint64_t* d_find = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq.p;
   auto fetch_per_doc = [&]() -> int {
     if (!dv) {
       CK(cudaMemcpyAsync(flags, w.d_doc_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
@@ -1885,9 +1915,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     if (total > cap) return ACG_E_OVERFLOW;
     if (total) {
       if (!out) return ACG_E_INVALID_ARG;
-      if (!dv && (rc = ensure_seq(w, total))) return rc;
+      if (!dv && (rc = reserve_seq(w, total))) return rc;
       p.incl = d_incl;
-      p.out = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq;
+      p.out = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq.p;
       p.cap = total;
       CK(acb::launch_seq_docs(a->dev, p, w.stream));
       w.stats.launches += 1;
@@ -1920,10 +1950,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     // best match at the smallest start; mode 2: the smallest end, longest first, then list order -- entry 0 of
     // the first match state entered), the first tuple acg_find takes from the same keys in sorted order.
     acb::DocFlagsLaunch f;
-    f.keys = w.d_keys[r.sorted_buf];
-    f.pids = w.d_pids[r.sorted_buf];
-    f.pattern_lens = a->d_plens;
-    f.n = r.n;
+    f.t = tuple_list(a, w, r);
     f.mode = chain_mode;
     f.span_start = span_start;
     f.doc_offsets = d_offs;
@@ -1955,10 +1982,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     CK(cudaMemsetAsync(dv->match_offsets, 0, nd1 * 8, w.stream));
   } else {
     acb::DocRecordsLaunch e;
-    e.keys = w.d_keys[r.sorted_buf];
-    e.pids = w.d_pids[r.sorted_buf];
-    e.pattern_lens = a->d_plens;
-    e.n = r.n;
+    e.t = tuple_list(a, w, r);
     e.mode = chain_mode;
     e.span_start = span_start;
     e.doc_offsets = d_offs;
@@ -2370,83 +2394,7 @@ int acg_find_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len,
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,
              uint64_t span_end, int anchored, int earliest, acg_match* out, int* found) {
-  if (!out || !found) return ACG_E_INVALID_ARG;
-  *found = 0;
-  int rc = validate_common(a, hay_len, span_start, span_end, anchored);
-  if (rc) return rc;
-  if ((rc = check_start(a->h, anchored))) return rc;
-  if (!a->on_device) return ACG_E_NO_DEVICE;
-  if (span_start > span_end) return ACG_OK;
-  earliest = find_earliest(a, anchored, earliest);
-  DeviceGuard guard(a->device);
-  WsLease lease(a);
-  if (lease.rc) return lease.rc;
-  Workspace& w = cur_ws();
-  const int engine = choose_engine(a, anchored, earliest, ACG_ENGINE_SEQUENTIAL, false);
-  w.stats.engine = engine;
-  // the prefilter engine's window-by-window copy below only takes the room
-  Placement pl;
-  if ((rc = place_input(a, hay, false, hay_len, span_start, span_end, engine == ACG_ENGINE_PREFILTER, &pl))) return rc;
-  if (engine == ACG_ENGINE_SEQUENTIAL) {
-    uint64_t n = 0;
-    rc = run_seq(a, pl.base, span_start, span_end, anchored, earliest, 1, out, 1, &n);
-    if (rc == ACG_OK && n) *found = 1;
-    return rc;
-  }
-  // The reference's try_find is lazy (it stops reading at the first match, SURVEY.md section
-  // 7h); the eager device scan therefore works through geometrically growing windows of start
-  // offsets (1 MiB, 16 MiB, 256 MiB, ...), copying only what a window needs.
-  const int mode = a->h.match_kind == ACG_STANDARD ? 0 : 1;
-  const uint64_t look = a->h.max_pattern_len + 64;
-  uint64_t copied_hi = span_start;
-  // Scan the start offsets [lo, hi) and fetch the first tuple (*n: the number of tuples).
-  auto first_in = [&](uint64_t lo, uint64_t hi, uint64_t* key, uint32_t* pid, uint64_t* n) -> int {
-    const uint64_t upto = std::min(hi + look, span_end);
-    if (upto > copied_hi) {
-      CK(cudaMemcpyAsync(const_cast<uint8_t*>(pl.base) + copied_hi, hay + copied_hi, upto - copied_hi,
-                         cudaMemcpyHostToDevice, w.stream));
-      copied_hi = upto;
-    }
-    TupleResult r;
-    int rc = run_prefilter(a, pl.base, copied_hi == span_end ? span_end + 32 : copied_hi, span_start, span_end,
-                           mode == 0 ? 2 : 1, &r, nullptr, lo, hi);
-    *n = r.n;
-    if (rc || r.n == 0) return rc;
-    CK(cudaMemcpyAsync(w.h_counter, w.d_keys[r.sorted_buf], 8, cudaMemcpyDeviceToHost, w.stream));
-    CK(cudaMemcpyAsync(w.h_counter + 1, w.d_pids[r.sorted_buf], 4, cudaMemcpyDeviceToHost, w.stream));
-    CK(cudaStreamSynchronize(w.stream));
-    *key = w.h_counter[0];
-    *pid = uint32_t(w.h_counter[1]);
-    return ACG_OK;
-  };
-  const uint32_t* plens = a->h.pattern_lens.data();
-  uint64_t lo = span_start, win = 1ull << 20;
-  while (lo < span_end) {
-    const uint64_t hi = std::min(span_end, lo + win);
-    uint64_t key = 0, n = 0;
-    uint32_t pid = 0;
-    if ((rc = first_in(lo, hi, &key, &pid, &n))) return rc;
-    if (n) {
-      const uint64_t end = acb::decode_key(key, pid, mode, span_start, plens).end;
-      if (mode == 0 && end > hi && hi < span_end) {
-        // Standard: a match that starts in [hi, end) could still end earlier -- scan those starts
-        uint64_t key2 = 0, n2 = 0;
-        uint32_t pid2 = 0;
-        if ((rc = first_in(hi, std::min(span_end, end), &key2, &pid2, &n2))) return rc;
-        if (n2 && key2 < key) { key = key2; pid = pid2; }
-      }
-      const acb::MatchSpan m = acb::decode_key(key, pid, mode, span_start, plens);
-      out->pid = pid;
-      out->_pad = 0;
-      out->start = m.start;
-      out->end = m.end;
-      *found = 1;
-      return ACG_OK;
-    }
-    lo = hi;
-    win = std::min<uint64_t>(win * 16, 1ull << 30);
-  }
-  return ACG_OK;
+  return find_impl(a, hay, hay_len, span_start, span_end, anchored, earliest, out, found);
 }
 
 // ---- packed searcher (src/packed/api.rs) ----------------------------------------------------

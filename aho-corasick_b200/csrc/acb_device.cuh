@@ -30,6 +30,14 @@ __host__ __device__ __forceinline__ MatchSpan decode_key(uint64_t key, uint32_t 
   return MatchSpan{at - pattern_lens[pid], at};
 }
 
+// The ordered tuples a search left in the workspace: first member of every launch struct that reads them.
+struct TupleList {
+  const uint64_t* keys;
+  const uint32_t* pids;
+  const uint32_t* pattern_lens;
+  uint64_t n;
+};
+
 struct DfaDev {
   const uint32_t* trans;          // premultiplied ids, as shipped (src/dfa.rs:92-95)
   const uint8_t* classes;         // [256] byte -> class (src/util/alphabet.rs)
@@ -119,10 +127,7 @@ cudaError_t inclusive_sum_u64(void* d_temp, size_t& temp_bytes, const unsigned l
 // since the keys of one document order its candidates as try_find prefers them -- written at out[doc * 3] in
 // the acg_doc_match layout, flags[doc] = found; (0 | doc << 32, 0, 0) and 0 for a document without one.
 struct DocFlagsLaunch {
-  const uint64_t* keys;
-  const uint32_t* pids;
-  const uint32_t* pattern_lens;
-  uint64_t n;
+  TupleList t;
   int mode;                     // key layout as ChainLaunch::mode
   uint64_t span_start;
   const uint64_t* doc_offsets;  // [n_docs + 1]
@@ -141,10 +146,7 @@ cudaError_t launch_doc_first(const DocFlagsLaunch& f, cudaStream_t s);
 // (match_offsets[n_docs] = n).  Record i writes match_offsets[d] = i for every d in (doc of i - 1, doc of i], the
 // last one also (doc of n - 1, n_docs]: every entry is written once, with no atomics.  n > 0.
 struct DocRecordsLaunch {
-  const uint64_t* keys;
-  const uint32_t* pids;
-  const uint32_t* pattern_lens;
-  uint64_t n;
+  TupleList t;
   int mode;                     // key layout as ChainLaunch::mode
   uint64_t span_start;
   const uint64_t* doc_offsets;  // [n_docs + 1]
@@ -225,10 +227,7 @@ cudaError_t launch_bytescan(const DfaDev& dfa, const PrefilterLaunch& p, int sm_
 // mode 0 (standard): keys = (end_rel << 24 | tie), sorted by (end, len desc, list order).
 // Writes flags[i] = 1 for the tuples the reference's iterator would yield.
 struct ChainLaunch {
-  const uint64_t* keys;
-  const uint32_t* pids;
-  const uint32_t* pattern_lens;
-  uint64_t n;
+  TupleList t;
   int mode;
   uint64_t* scratch_end;   // [n] end offsets (leftmost) -> inclusive prefix max
   uint8_t* flags;          // [n]
@@ -244,10 +243,7 @@ cudaError_t select_flagged(void* d_temp, size_t& temp_bytes, const uint64_t* key
 // keeping only ends > min_end (writes compacted output; order preserved because kept tuples are a
 // suffix of the end-sorted list).
 struct ExpandLaunch {
-  const uint64_t* keys;
-  const uint32_t* pids;
-  const uint32_t* pattern_lens;
-  uint64_t n;
+  TupleList t;
   uint64_t first;        // index of the first kept tuple (host-side binary search result)
   uint64_t span_start;
   uint64_t offset_add;

@@ -312,16 +312,16 @@ __device__ __forceinline__ uint64_t doc_of(const uint64_t* offs, uint64_t n_docs
 
 // The haystack offsets of tuple i.
 __device__ __forceinline__ MatchSpan tuple_span(const DocFlagsLaunch& f, uint64_t i) {
-  return decode_key(f.keys[i], f.pids[i], f.mode, f.span_start, f.pattern_lens);
+  return decode_key(f.t.keys[i], f.t.pids[i], f.mode, f.span_start, f.t.pattern_lens);
 }
 
 // Over the n tuples of a prefilter scan.  is_match: flags[doc] = 1 for the document of every tuple.
 // find (best != nullptr): best[doc] = the smallest key of the document's tuples.
 __global__ void doc_flags_kernel(DocFlagsLaunch f) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= f.n) return;
+  if (i >= f.t.n) return;
   const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, tuple_span(f, i).start);
-  if (f.best) atomicMin(f.best + doc, (unsigned long long)f.keys[i]);
+  if (f.best) atomicMin(f.best + doc, (unsigned long long)f.t.keys[i]);
   else f.flags[doc] = 1;
 }
 
@@ -341,12 +341,12 @@ __global__ void doc_first_clear_kernel(DocFlagsLaunch f) {
 // a document, so one tuple per document writes.
 __global__ void doc_first_kernel(DocFlagsLaunch f) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= f.n) return;
+  if (i >= f.t.n) return;
   const MatchSpan m = tuple_span(f, i);
   const uint64_t doc = doc_of(f.doc_offsets, f.n_docs, m.start);
-  if (f.keys[i] != f.best[doc]) return;
+  if (f.t.keys[i] != f.best[doc]) return;
   const uint64_t base = f.doc_offsets[doc];
-  f.out[doc * 3 + 0] = (uint64_t)f.pids[i] | doc << 32;
+  f.out[doc * 3 + 0] = (uint64_t)f.t.pids[i] | doc << 32;
   f.out[doc * 3 + 1] = m.start - base;
   f.out[doc * 3 + 2] = m.end - base;
   f.flags[doc] = 1;
@@ -356,19 +356,19 @@ __global__ void doc_first_kernel(DocFlagsLaunch f) {
 // DocRecordsLaunch).  No match crosses a document end, so the documents of the records do not decrease.
 __global__ void doc_records_kernel(DocRecordsLaunch e) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= e.n) return;
-  const uint32_t pid = e.pids[i];
-  const MatchSpan m = decode_key(e.keys[i], pid, e.mode, e.span_start, e.pattern_lens);
+  if (i >= e.t.n) return;
+  const uint32_t pid = e.t.pids[i];
+  const MatchSpan m = decode_key(e.t.keys[i], pid, e.mode, e.span_start, e.t.pattern_lens);
   const uint64_t doc = doc_of(e.doc_offsets, e.n_docs, m.start);
   const uint64_t base = e.doc_offsets[doc];
   e.out[i * 3 + 0] = (uint64_t)pid | doc << 32;
   e.out[i * 3 + 1] = m.start - base;
   e.out[i * 3 + 2] = m.end - base;
   uint64_t d = 0;
-  if (i) d = doc_of(e.doc_offsets, e.n_docs, decode_key(e.keys[i - 1], e.pids[i - 1], e.mode, e.span_start, e.pattern_lens).start) + 1;
+  if (i) d = doc_of(e.doc_offsets, e.n_docs, decode_key(e.t.keys[i - 1], e.t.pids[i - 1], e.mode, e.span_start, e.t.pattern_lens).start) + 1;
   for (; d <= doc; ++d) e.match_offsets[d] = i;
-  if (i + 1 == e.n)
-    for (d = doc + 1; d <= e.n_docs; ++d) e.match_offsets[d] = e.n;
+  if (i + 1 == e.t.n)
+    for (d = doc + 1; d <= e.n_docs; ++d) e.match_offsets[d] = e.t.n;
 }
 
 __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
@@ -390,13 +390,13 @@ __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint
 template <int kExpandThreads>
 __global__ void __launch_bounds__(kExpandThreads) expand_kernel(ExpandLaunch e) {
   __shared__ uint64_t s_rec[kExpandThreads * 3];
-  const uint64_t m = e.n - e.first;
+  const uint64_t m = e.t.n - e.first;
   // grid-stride over blocks of kExpandThreads records (the small form runs one CTA per SM)
   for (uint64_t base = (uint64_t)blockIdx.x * kExpandThreads; base < m; base += (uint64_t)gridDim.x * kExpandThreads) {
     const uint64_t i = base + threadIdx.x;
     if (i < m) {
-      const uint32_t pid = e.pids[e.first + i];
-      const MatchSpan span = decode_key(e.keys[e.first + i], pid, 0, e.span_start + e.offset_add, e.pattern_lens);
+      const uint32_t pid = e.t.pids[e.first + i];
+      const MatchSpan span = decode_key(e.t.keys[e.first + i], pid, 0, e.span_start + e.offset_add, e.t.pattern_lens);
       s_rec[threadIdx.x * 3 + 0] = (uint64_t)pid;
       s_rec[threadIdx.x * 3 + 1] = span.start;
       s_rec[threadIdx.x * 3 + 2] = span.end;
@@ -431,7 +431,7 @@ __global__ void lower_bound_kernel(const uint64_t* keys, uint64_t n, uint64_t bo
 }  // namespace
 
 cudaError_t launch_expand(const ExpandLaunch& e, cudaStream_t s) {
-  const uint64_t m = e.n - e.first;
+  const uint64_t m = e.t.n - e.first;
   if (m == 0) return cudaSuccess;
   if (e.small) {
     // one small CTA per SM at most: the persistent scan CTA of the next step must still fit beside it
@@ -473,23 +473,23 @@ cudaError_t launch_seq_docs(const DfaDev& dfa, const SeqDocsLaunch& p, cudaStrea
 }
 
 cudaError_t launch_doc_flags(const DocFlagsLaunch& f, cudaStream_t s) {
-  if (f.n == 0) return cudaSuccess;
-  ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
+  if (f.t.n == 0) return cudaSuccess;
+  ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.t.n + 255) / 256), 256, 0, s, f);
   return cudaGetLastError();
 }
 
 cudaError_t launch_doc_first(const DocFlagsLaunch& f, cudaStream_t s) {
   if (f.n_docs == 0) return cudaSuccess;
   ACB_LAUNCH(doc_first_clear_kernel, (unsigned)((f.n_docs + 255) / 256), 256, 0, s, f);
-  if (f.n == 0) return cudaGetLastError();
-  ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
-  ACB_LAUNCH(doc_first_kernel, (unsigned)((f.n + 255) / 256), 256, 0, s, f);
+  if (f.t.n == 0) return cudaGetLastError();
+  ACB_LAUNCH(doc_flags_kernel, (unsigned)((f.t.n + 255) / 256), 256, 0, s, f);
+  ACB_LAUNCH(doc_first_kernel, (unsigned)((f.t.n + 255) / 256), 256, 0, s, f);
   return cudaGetLastError();
 }
 
 cudaError_t launch_doc_records(const DocRecordsLaunch& e, cudaStream_t s) {
-  if (e.n == 0) return cudaSuccess;
-  ACB_LAUNCH(doc_records_kernel, (unsigned)((e.n + 255) / 256), 256, 0, s, e);
+  if (e.t.n == 0) return cudaSuccess;
+  ACB_LAUNCH(doc_records_kernel, (unsigned)((e.t.n + 255) / 256), 256, 0, s, e);
   return cudaGetLastError();
 }
 

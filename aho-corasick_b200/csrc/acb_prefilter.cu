@@ -944,19 +944,19 @@ __global__ void __launch_bounds__(kBsThreads, 2) bytescan_kernel(DfaDev d, Prefi
 // ---- chain resolution ---------------------------------------------------------
 
 __device__ __forceinline__ void tuple_span(const ChainLaunch& c, uint64_t i, uint64_t* s, uint64_t* e) {
-  const uint64_t key = c.keys[i];
+  const uint64_t key = c.t.keys[i];
   if (c.mode == 1) {
     *s = key >> kTieBits;
     *e = *s + (key & kTieMask);
   } else {
     *e = key >> kTieBits;
-    *s = *e - c.pattern_lens[c.pids[i]];
+    *s = *e - c.t.pattern_lens[c.t.pids[i]];
   }
 }
 
 __global__ void chain_ends_kernel(ChainLaunch c) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c.n) return;
+  if (i >= c.t.n) return;
   uint64_t s, e;
   tuple_span(c, i, &s, &e);
   c.scratch_end[i] = e;
@@ -968,13 +968,13 @@ __global__ void chain_ends_kernel(ChainLaunch c) {
 // anchor's thread resolves the short run of mutually overlapping tuples after it.
 __global__ void chain_select_kernel(ChainLaunch c) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c.n) return;
+  if (i >= c.t.n) return;
   uint64_t s, e;
   tuple_span(c, i, &s, &e);
   if (i > 0 && c.scratch_end[i - 1] > s) return;  // not an anchor: an earlier anchor's thread decides
   c.flags[i] = 1;
   uint64_t cur_end = e;
-  for (uint64_t j = i + 1; j < c.n; ++j) {
+  for (uint64_t j = i + 1; j < c.t.n; ++j) {
     uint64_t sj, ej;
     tuple_span(c, j, &sj, &ej);
     if (c.scratch_end[j - 1] <= sj) break;  // next anchor
@@ -1219,12 +1219,12 @@ cudaError_t launch_bytescan(const DfaDev& dfa, const PrefilterLaunch& p, int sm_
 }
 
 cudaError_t launch_chain_ends(const ChainLaunch& c, cudaStream_t s) {
-  const unsigned blocks = (unsigned)((c.n + 255) / 256);
+  const unsigned blocks = (unsigned)((c.t.n + 255) / 256);
   ACB_LAUNCH(chain_ends_kernel, blocks, 256, 0, s, c);
   return cudaGetLastError();
 }
 cudaError_t launch_chain_select(const ChainLaunch& c, cudaStream_t s) {
-  const unsigned blocks = (unsigned)((c.n + 255) / 256);
+  const unsigned blocks = (unsigned)((c.t.n + 255) / 256);
   ACB_LAUNCH(chain_select_kernel, blocks, 256, 0, s, c);
   return cudaGetLastError();
 }

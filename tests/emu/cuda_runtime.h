@@ -13,6 +13,7 @@
 #include <ucontext.h>
 
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cstdint>
 #include <cstdio>
@@ -66,17 +67,32 @@ inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) {
   *v = e ? std::atoi(e) : 3;  // few "SMs": fewer CTAs to run one after the other, still several chunks
   return cudaSuccess;
 }
+// Allocation calls seen so far and, for tests of what a failed grow leaves behind, the call that is to fail:
+// [0] cudaMalloc, [1] cudaMallocHost.  acb_emu_fail_alloc(host, n): the n-th call from now fails, once.
+namespace emu_alloc {
+inline std::atomic<long> calls[2], fail_in[2];
+inline bool fails(int host) {
+  ++calls[host];
+  return fail_in[host].load() > 0 && fail_in[host].fetch_sub(1) == 1;
+}
+}  // namespace emu_alloc
+extern "C" __attribute__((used)) inline long acb_emu_alloc_calls(int host) { return emu_alloc::calls[host]; }
+extern "C" __attribute__((used)) inline void acb_emu_fail_alloc(int host, long nth) { emu_alloc::fail_in[host] = nth; }
 template <class T>
 inline cudaError_t cudaMalloc(T** p, size_t n) {
   void* q = nullptr;
-  if (posix_memalign(&q, 256, n ? n : 1)) return cudaErrorMemoryAllocation;
+  if (emu_alloc::fails(0) || posix_memalign(&q, 256, n ? n : 1)) return cudaErrorMemoryAllocation;
   std::memset(q, 0xCD, n);  // device memory is not zero-initialised
   *p = static_cast<T*>(q);
   return cudaSuccess;
 }
 inline cudaError_t cudaFree(void* p) { std::free(p); return cudaSuccess; }
 template <class T>
-inline cudaError_t cudaMallocHost(T** p, size_t n) { *p = static_cast<T*>(std::malloc(n ? n : 1)); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+inline cudaError_t cudaMallocHost(T** p, size_t n) {
+  if (emu_alloc::fails(1)) return cudaErrorMemoryAllocation;
+  *p = static_cast<T*>(std::malloc(n ? n : 1));
+  return *p ? cudaSuccess : cudaErrorMemoryAllocation;
+}
 inline cudaError_t cudaFreeHost(void* p) { std::free(p); return cudaSuccess; }
 inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { if (n) std::memmove(d, s, n); return cudaSuccess; }
 inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { if (n) std::memmove(d, s, n); return cudaSuccess; }
