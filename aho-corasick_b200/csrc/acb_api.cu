@@ -92,13 +92,11 @@ struct Workspace {
   DevBuf<unsigned long long> d_counter;
   PinnedBuf<unsigned long long> h_counter;
   DevBuf<uint8_t> d_temp;  // CUB temporary storage (cub_call): a search's CUB calls run in order on `stream`
-  PinnedBuf<uint64_t> h_keys;  // staging of the tuples on their way to the caller
-  PinnedBuf<uint32_t> h_pids;
   DevBuf<uint8_t> d_hay;  // staging of host haystacks
   DevBuf<uint64_t> d_scratch;  // chain resolution: end offsets / prefix max
   DevBuf<uint8_t> d_flags;
-  DevBuf<uint64_t> d_seq;  // sequential engine output, three words per record
-  PinnedBuf<uint64_t> h_seq;
+  DevBuf<uint64_t> d_rec;  // records of a host-output search, three words each, and their staging on the host
+  PinnedBuf<uint64_t> h_rec;
   acg_stats stats{};  // of the search that holds (or last held) this workspace
   // pageable host haystacks: page-locked staging ring filled by host threads (run_prefilter)
   PinnedBuf<uint8_t> h_stage[2];
@@ -756,10 +754,11 @@ int cub_call(Workspace& w, F f) {
   return ACG_OK;
 }
 
-// sequential engine, batched find: room for `cap` records on the device and on their way to the caller
-int reserve_seq(Workspace& w, uint64_t cap) {
-  int rc = w.d_seq.reserve(cap * 3);
-  return rc ? rc : w.h_seq.reserve(cap * 3);
+// host output: room for n records on the device and on their way to the caller
+int reserve_rec(Workspace& w, uint64_t n) {
+  n = std::max<uint64_t>(n, 1 << 16) * 3;
+  int rc = w.d_rec.reserve(n);
+  return rc ? rc : w.h_rec.reserve(n);
 }
 
 // batched search: room for n entries in each per-document array
@@ -1256,54 +1255,26 @@ int run_chain(const acg_dfa* a, int mode, TupleResult* r) {
   return ACG_OK;
 }
 
-// D2H + expansion of ordered (key,pid) tuples into acg_match / count / fnv.  Batched search (`docs`,
-// the host CSR offsets): acg_doc_match records -- the document in the pad, offsets relative to it.  No
-// match crosses a document end, so the ordered tuples are document-major and one forward walk over the
-// offsets tags them.
-int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, acg_match* out,
-                 uint64_t cap, uint64_t* n_out, uint64_t* fnv, int key_mode = 0, const uint64_t* docs = nullptr) {
+// Host output: the n records the device wrote to w.d_rec, copied to the caller's `out` through their page-locked
+// staging -- or, for count_overlapping (`fnv`), only the FNV-1a of their words.  The time from ev0, which the
+// caller records before the records are written, to the end of the copy goes to d2h_ms.
+int copy_out(uint64_t n, acg_match* out, uint64_t* fnv) {
   Workspace& w = cur_ws();
-  *n_out = r.n;
-  if (fnv) *fnv = 0xcbf29ce484222325ull;
-  if (r.n == 0) return ACG_OK;
-  if (!fnv && r.n > cap) return ACG_E_OVERFLOW;
-  int rc = reserve_all(std::max<uint64_t>(r.n, 1 << 16), w.h_keys, w.h_pids);
-  if (rc) return rc;
-  const acb::TupleList t = tuple_list(a, w, r);
-  CK(cudaEventRecord(w.ev0, w.stream));
-  CK(cudaMemcpyAsync(w.h_keys, t.keys, r.n * 8, cudaMemcpyDeviceToHost, w.stream));
-  CK(cudaMemcpyAsync(w.h_pids, t.pids, r.n * 4, cudaMemcpyDeviceToHost, w.stream));
+  if (n) CK(cudaMemcpyAsync(w.h_rec, w.d_rec, n * 24, cudaMemcpyDeviceToHost, w.stream));
   CK(cudaEventRecord(w.ev1, w.stream));
   CK(cudaStreamSynchronize(w.stream));
   float ms = 0;
   cudaEventElapsedTime(&ms, w.ev0, w.ev1);
-  cur_ws().stats.d2h_ms += ms;
-  const uint32_t* plens = a->h.pattern_lens.data();
-  uint64_t hsh = 0xcbf29ce484222325ull;
-  auto mix = [&](uint64_t v) {
-    for (int k = 0; k < 8; ++k) { hsh ^= (v >> (8 * k)) & 0xFF; hsh *= 0x100000001b3ull; }
-  };
-  uint32_t doc = 0;
-  for (uint64_t i = 0; i < r.n; ++i) {
-    const uint32_t pid = w.h_pids[i];
-    const acb::MatchSpan m = acb::decode_key(w.h_keys[i], pid, key_mode, span_start, plens);
-    uint64_t start = m.start, end = m.end;
-    if (docs) {
-      while (docs[doc + 1] <= start) ++doc;
-      start -= docs[doc];
-      end -= docs[doc];
-    }
-    if (out && i < cap) {
-      out[i].pid = pid;
-      out[i]._pad = doc;
-      out[i].start = start;
-      out[i].end = end;
-    }
-    if (fnv) { mix(pid); mix(start); mix(end); }
+  w.stats.d2h_ms += ms;
+  if (fnv) {
+    uint64_t hsh = 0xcbf29ce484222325ull;
+    for (uint64_t i = 0; i < n * 3; ++i)
+      for (int k = 0; k < 8; ++k) { hsh ^= (w.h_rec[i] >> (8 * k)) & 0xFF; hsh *= 0x100000001b3ull; }
+    *fnv = hsh;
+  } else if (n) {
+    CopyPool::get().copy(reinterpret_cast<uint8_t*>(out), reinterpret_cast<const uint8_t*>(w.h_rec.p), n * 24);
   }
-  if (fnv) *fnv = hsh;
-  if (out == nullptr && !fnv) return ACG_E_INVALID_ARG;
-  return (out && r.n > cap) ? ACG_E_OVERFLOW : ACG_OK;
+  return ACG_OK;
 }
 
 // The sequential engine over [span_start, span_end): the one-document form of seq_docs_kernel, which counts
@@ -1311,13 +1282,13 @@ int drain_tuples(const acg_dfa* a, const TupleResult& r, uint64_t span_start, ac
 int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_t span_end,
             int anchored, int earliest, int single, acg_match* out, uint64_t cap, uint64_t* n_out) {
   Workspace& w = cur_ws();
-  uint64_t scap = std::max<uint64_t>(std::max<uint64_t>(cap, 1024), w.d_seq.cap / 3);
+  uint64_t scap = cap;
   int rc = reserve_docs(w, 2);
   if (rc) return rc;
   const uint64_t bounds[2] = {span_start, span_end};
   CK(cudaMemcpyAsync(w.d_doc_offs, bounds, sizeof(bounds), cudaMemcpyHostToDevice, w.stream));
   for (int attempt = 0; attempt < 4; ++attempt) {
-    if ((rc = reserve_seq(w, scap))) return rc;
+    if ((rc = reserve_rec(w, scap))) return rc;
     acb::SeqDocsLaunch p{};
     p.hay = d_hay;
     p.doc_offsets = w.d_doc_offs;
@@ -1327,8 +1298,8 @@ int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_
     p.earliest = earliest;
     p.single = single;
     p.counts = w.d_counter;
-    p.out = w.d_seq;
-    p.cap = w.d_seq.cap / 3;
+    p.out = w.d_rec;
+    p.cap = w.d_rec.cap / 3;
     CK(cudaEventRecord(w.ev0, w.stream));
     CK(acb::launch_seq_docs(a->dev, p, w.stream));
     CK(cudaEventRecord(w.ev1, w.stream));
@@ -1342,15 +1313,15 @@ int run_seq(const acg_dfa* a, const uint8_t* d_hay, uint64_t span_start, uint64_
     *n_out = n;
     cur_ws().stats.raw_matches = n;
     if (n > cap) return ACG_E_OVERFLOW;  // caller retries with a bigger buffer (two-call protocol)
-    if (n > w.d_seq.cap / 3) { scap = n; continue; }
+    if (n > w.d_rec.cap / 3) { scap = n; continue; }
     if (n) {
-      CK(cudaMemcpyAsync(w.h_seq, w.d_seq, n * 24, cudaMemcpyDeviceToHost, w.stream));
+      CK(cudaMemcpyAsync(w.h_rec, w.d_rec, n * 24, cudaMemcpyDeviceToHost, w.stream));
       CK(cudaStreamSynchronize(w.stream));
       for (uint64_t i = 0; i < n; ++i) {
-        out[i].pid = uint32_t(w.h_seq[i * 3]);
+        out[i].pid = uint32_t(w.h_rec[i * 3]);
         out[i]._pad = 0;
-        out[i].start = span_start + w.h_seq[i * 3 + 1];
-        out[i].end = span_start + w.h_seq[i * 3 + 2];
+        out[i].start = span_start + w.h_rec[i * 3 + 1];
+        out[i].end = span_start + w.h_rec[i * 3 + 2];
       }
     }
     return ACG_OK;
@@ -1475,6 +1446,36 @@ int scan_overlapping(const acg_dfa* a, const uint8_t* hay, bool on_device, uint6
   return ACG_OK;
 }
 
+// The records of the ordered tuples of r from index `first` on (key layout `mode`), expanded into the caller's
+// device buffer (`devout`), or into the workspace and copied to the host `out` -- count_overlapping (`fnv`) only
+// hashes them.  On overflow nothing is written: the caller retries with room for *n_out.
+int expand_out(const acg_dfa* a, const TupleResult& r, uint64_t first, int mode, uint64_t span_start,
+               const DevOut* devout, acg_match* out, uint64_t cap, uint64_t* n_out, uint64_t* fnv) {
+  Workspace& w = cur_ws();
+  const uint64_t n = r.n - first;
+  *n_out = n;
+  if (!fnv && n > cap) return ACG_E_OVERFLOW;
+  if (!devout && !fnv && n && !out) return ACG_E_INVALID_ARG;
+  int rc = devout ? ACG_OK : reserve_rec(w, n);
+  if (rc) return rc;
+  acb::ExpandLaunch e;
+  e.t = tuple_list(a, w, r);
+  e.first = first;
+  e.mode = mode;
+  e.span_start = span_start;
+  e.offset_add = devout ? devout->offset_add : 0;
+  e.out = devout ? static_cast<uint64_t*>(devout->d_out) : w.d_rec.p;
+  CK(cudaEventRecord(w.ev0, w.stream));
+  CK(acb::launch_expand(e, w.stream));
+  if (!devout) {
+    w.stats.launches += 1;
+    return copy_out(n, out, fnv);
+  }
+  CK(cudaStreamSynchronize(w.stream));
+  w.stats.launches += 2;
+  return ACG_OK;
+}
+
 int overlapping_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                      uint64_t span_start, uint64_t span_end, int anchored, acg_match* out,
                      uint64_t cap, uint64_t* n_out, uint64_t* fnv, float* kernel_ms,
@@ -1500,23 +1501,7 @@ int overlapping_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, u
                              &r, &first)))
     return rc;
   if (kernel_ms) *kernel_ms = cur_ws().stats.scan_ms + cur_ws().stats.order_ms;
-  if (devout) {
-    Workspace& w = cur_ws();
-    const uint64_t kept = r.n - first;
-    *n_out = kept;
-    if (kept > cap) return ACG_E_OVERFLOW;
-    acb::ExpandLaunch e;
-    e.t = tuple_list(a, w, r);
-    e.first = first;
-    e.span_start = span_start;
-    e.offset_add = devout->offset_add;
-    e.out = static_cast<uint64_t*>(devout->d_out);
-    CK(acb::launch_expand(e, w.stream));
-    CK(cudaStreamSynchronize(w.stream));
-    cur_ws().stats.launches += 2;
-    return ACG_OK;
-  }
-  return drain_tuples(a, r, span_start, out, cap, n_out, fnv);
+  return expand_out(a, r, first, 0, span_start, devout, out, cap, n_out, fnv);
 }
 
 // acg_shard_plan: the slice arithmetic shared by every rank (SURVEY.md section 8e).  Interior
@@ -1595,6 +1580,7 @@ int sharded_begin(const acg_dfa* a, acg_comm* c, const uint8_t* hay, bool hay_on
     acb::ExpandLaunch e;
     e.t = tuple_list(a, w, r);
     e.first = first;
+    e.mode = 0;
     e.span_start = lspan_s;
     e.offset_add = hay_off;
     e.out = reinterpret_cast<uint64_t*>(target);
@@ -1699,7 +1685,7 @@ int find_iter_impl(const acg_dfa* a, const uint8_t* hay, bool hay_on_device, uin
   if ((rc = run_prefilter(a, pl.base, pl.readable, span_start, span_end, mode == 0 ? 2 : 1, &r, pl.h_src))) return rc;
   if ((rc = run_chain(a, mode, &r))) return rc;
   if (kernel_ms) *kernel_ms = cur_ws().stats.scan_ms + cur_ws().stats.order_ms;
-  return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, mode);
+  return expand_out(a, r, 0, mode, span_start, nullptr, out, cap, n_out, nullptr);
 }
 
 // acg_find (include/acb200.h)
@@ -1833,11 +1819,26 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   w.stats.engine = engine;
   const uint64_t nd1 = n_docs + 1;
   if ((rc = reserve_docs(w, nd1))) return rc;
-  if (what == kBatchFind && !dv && (rc = reserve_seq(w, n_docs))) return rc;  // the records, at index doc
   uint64_t span_start, span_end;
   const uint64_t* d_offs = w.d_doc_offs;
   unsigned long long* const d_counts = w.d_doc_counts;
   unsigned long long* const d_incl = w.d_doc_incl;
+  // The results go to the caller's device arrays, or to the workspace's and from there to the host at the end.
+  // The records (find: one per document, at index doc) get their place once their number is known; on overflow
+  // nothing is written, and the caller retries with room for *n_out.
+  uint8_t* const d_flags = dv ? flags : w.d_doc_flags.p;
+  uint64_t* const d_index = dv ? dv->match_offsets : reinterpret_cast<uint64_t*>(d_counts);
+  uint64_t* d_rec = nullptr;
+  uint64_t n_rec = 0;
+  auto records = [&](uint64_t n) -> int {
+    if (n > cap) return ACG_E_OVERFLOW;
+    if (n && !out) return ACG_E_INVALID_ARG;
+    n_rec = n;
+    const int e = dv ? ACG_OK : reserve_rec(w, n);
+    d_rec = dv ? reinterpret_cast<uint64_t*>(out) : w.d_rec.p;
+    return e;
+  };
+  if (what == kBatchFind && (rc = records(n_docs))) return rc;
   if (offs_on_device) {
     // checked where they are; the span bounds come back with the verdict (placement and the scan plan need them)
     CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
@@ -1861,18 +1862,21 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   }
   Placement pl;
   if ((rc = place_input(a, hay, hay_on_device, hay_len, span_start, span_end, use_pf, &pl))) return rc;
-  // per-document results: the caller's device arrays, or the workspace's and a copy to the host
-  uint8_t* d_flags = dv ? flags : w.d_doc_flags;
-  uint64_t* d_find = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq.p;
-  auto fetch_per_doc = [&]() -> int {
-    if (!dv) {
-      CK(cudaMemcpyAsync(flags, w.d_doc_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
-      if (what == kBatchFind) CK(cudaMemcpyAsync(out, w.d_seq, n_docs * 24, cudaMemcpyDeviceToHost, w.stream));
+  // The end of a batch: the time between ev2 and ev3 to `ms_to` -- the sequential engine's scan, the order time
+  // of the prefilter engine's per-document step -- and for host output the copy of the flags and the records.
+  auto finish = [&](float& ms_to) -> int {
+    if (dv) {
+      CK(cudaStreamSynchronize(w.stream));
+    } else {
+      CK(cudaEventRecord(w.ev0, w.stream));
+      if (per_doc) CK(cudaMemcpyAsync(flags, d_flags, n_docs, cudaMemcpyDeviceToHost, w.stream));
+      if (int e = copy_out(n_rec, out, nullptr)) return e;
     }
-    CK(cudaStreamSynchronize(w.stream));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+    ms_to += ms;
     return ACG_OK;
   };
-  float ms = 0;
   if (!use_pf) {
     // one thread per document: count, inclusive scan, fill at each document's offset
     acb::SeqDocsLaunch p{};
@@ -1884,21 +1888,18 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     p.overlapping = what == kBatchOverlapping;
     p.single = per_doc;
     p.earliest = what == kBatchIsMatch || earliest;
-    CK(cudaEventRecord(w.ev0, w.stream));
+    CK(cudaEventRecord(w.ev2, w.stream));
     if (per_doc) {
       p.flags = d_flags;
       if (what == kBatchFind) {
         p.find = 1;
-        p.out = d_find;
+        p.out = d_rec;
         p.cap = n_docs;
       }
       CK(acb::launch_seq_docs(a->dev, p, w.stream));
-      CK(cudaEventRecord(w.ev1, w.stream));
-      if ((rc = fetch_per_doc())) return rc;
-      cudaEventElapsedTime(&ms, w.ev0, w.ev1);
-      w.stats.scan_ms = ms;
+      CK(cudaEventRecord(w.ev3, w.stream));
       w.stats.launches += 1;
-      return ACG_OK;
+      return finish(w.stats.scan_ms);
     }
     p.counts = d_counts;
     CK(acb::launch_seq_docs(a->dev, p, w.stream));
@@ -1912,27 +1913,19 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     *n_out = total;
     w.stats.raw_matches = total;
     w.stats.launches += 2;
-    if (total > cap) return ACG_E_OVERFLOW;
+    if ((rc = records(total))) return rc;
     if (total) {
-      if (!out) return ACG_E_INVALID_ARG;
-      if (!dv && (rc = reserve_seq(w, total))) return rc;
       p.incl = d_incl;
-      p.out = dv ? reinterpret_cast<uint64_t*>(out) : w.d_seq.p;
+      p.out = d_rec;
       p.cap = total;
       CK(acb::launch_seq_docs(a->dev, p, w.stream));
       w.stats.launches += 1;
     }
-    CK(cudaEventRecord(w.ev1, w.stream));
-    if (dv) {  // the CSR index is the inclusive scan behind a zero
-      CK(cudaMemsetAsync(dv->match_offsets, 0, 8, w.stream));
-      CK(cudaMemcpyAsync(dv->match_offsets + 1, d_incl, n_docs * 8, cudaMemcpyDeviceToDevice, w.stream));
-    } else if (total) {
-      CK(cudaMemcpyAsync(out, w.d_seq, total * 24, cudaMemcpyDeviceToHost, w.stream));
-    }
-    CK(cudaStreamSynchronize(w.stream));
-    cudaEventElapsedTime(&ms, w.ev0, w.ev1);
-    w.stats.scan_ms = ms;
-    return ACG_OK;
+    CK(cudaEventRecord(w.ev3, w.stream));
+    // the CSR index is the inclusive scan behind a zero
+    CK(cudaMemsetAsync(d_index, 0, 8, w.stream));
+    CK(cudaMemcpyAsync(d_index + 1, d_incl, n_docs * 8, cudaMemcpyDeviceToDevice, w.stream));
+    return finish(w.stats.scan_ms);
   }
   // prefilter engine over the whole span, each match bounded by its document (PrefilterLaunch::doc_offsets)
   const int chain_mode = what == kBatchOverlapping || a->h.match_kind == ACG_STANDARD ? 0 : 1;
@@ -1959,7 +1952,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     CK(cudaEventRecord(w.ev2, w.stream));
     if (what == kBatchFind) {
       f.best = d_counts;
-      f.out = d_find;
+      f.out = d_rec;
       CK(acb::launch_doc_first(f, w.stream));
       w.stats.launches += 3;
     } else {
@@ -1968,18 +1961,14 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
       w.stats.launches += 1;
     }
     CK(cudaEventRecord(w.ev3, w.stream));
-    if ((rc = fetch_per_doc())) return rc;
-    cudaEventElapsedTime(&ms, w.ev2, w.ev3);
-    w.stats.order_ms = ms;
-    return ACG_OK;
+    return finish(w.stats.order_ms);
   }
   if (what == kBatchFindIter && (rc = run_chain(a, chain_mode, &r))) return rc;
-  if (!dv) return drain_tuples(a, r, span_start, out, cap, n_out, nullptr, chain_mode, offs);
   *n_out = r.n;
-  if (r.n > cap) return ACG_E_OVERFLOW;  // nothing written: the caller retries with room for *n_out
+  if ((rc = records(r.n))) return rc;
   CK(cudaEventRecord(w.ev2, w.stream));
   if (r.n == 0) {
-    CK(cudaMemsetAsync(dv->match_offsets, 0, nd1 * 8, w.stream));
+    CK(cudaMemsetAsync(d_index, 0, nd1 * 8, w.stream));
   } else {
     acb::DocRecordsLaunch e;
     e.t = tuple_list(a, w, r);
@@ -1987,16 +1976,13 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     e.span_start = span_start;
     e.doc_offsets = d_offs;
     e.n_docs = n_docs;
-    e.out = reinterpret_cast<uint64_t*>(out);
-    e.match_offsets = dv->match_offsets;
+    e.out = d_rec;
+    e.match_offsets = d_index;
     CK(acb::launch_doc_records(e, w.stream));
     w.stats.launches += 1;
   }
   CK(cudaEventRecord(w.ev3, w.stream));
-  CK(cudaStreamSynchronize(w.stream));
-  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
-  w.stats.order_ms += ms;
-  return ACG_OK;
+  return finish(w.stats.order_ms);
 }
 
 }  // namespace

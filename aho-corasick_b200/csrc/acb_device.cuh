@@ -239,12 +239,12 @@ cudaError_t select_flagged(void* d_temp, size_t& temp_bytes, const uint64_t* key
                            const uint8_t* flags, uint64_t* keys_out, uint32_t* pids_out,
                            unsigned long long* d_num_out, uint64_t n, cudaStream_t s);
 
-// Expand ordered (end_rel << 24 | tie, pid) tuples into 24-byte match records on the device,
-// keeping only ends > min_end (writes compacted output; order preserved because kept tuples are a
-// suffix of the end-sorted list).
+// Expand ordered (key, pid) tuples into 24-byte match records on the device, from tuple `first` on (sharded and
+// device-output overlapping searches: the ends > min_end, a suffix of the end-sorted list; order preserved).
 struct ExpandLaunch {
   TupleList t;
   uint64_t first;        // index of the first kept tuple (host-side binary search result)
+  int mode;              // key layout as ChainLaunch::mode
   uint64_t span_start;
   uint64_t offset_add;
   uint64_t* out;         // [ (n-first) * 3 ] as (pid, start, end) u64 triples == acg_match layout

@@ -396,7 +396,7 @@ __global__ void __launch_bounds__(kExpandThreads) expand_kernel(ExpandLaunch e) 
     const uint64_t i = base + threadIdx.x;
     if (i < m) {
       const uint32_t pid = e.t.pids[e.first + i];
-      const MatchSpan span = decode_key(e.t.keys[e.first + i], pid, 0, e.span_start + e.offset_add, e.t.pattern_lens);
+      const MatchSpan span = decode_key(e.t.keys[e.first + i], pid, e.mode, e.span_start + e.offset_add, e.t.pattern_lens);
       s_rec[threadIdx.x * 3 + 0] = (uint64_t)pid;
       s_rec[threadIdx.x * 3 + 1] = span.start;
       s_rec[threadIdx.x * 3 + 2] = span.end;

@@ -392,7 +392,8 @@ typedef struct {
   uint64_t raw_matches;      /* tuples appended before ordering/stitching */
   float scan_ms;             /* dominant scan kernel(s) */
   float order_ms;            /* ordering / compaction */
-  float h2d_ms, d2h_ms;
+  float h2d_ms;
+  float d2h_ms;              /* expansion of the records and their copy to the host */
 } acg_stats;
 int acg_last_stats(const acg_dfa* dfa, acg_stats* out);
 
