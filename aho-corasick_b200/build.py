@@ -8,7 +8,7 @@ HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 LIB = HERE / "libacb200.so"
 SOURCES = ["acb_build.cpp", "acb_kernels.cu", "acb_prefilter.cu", "acb_comm.cu", "acb_api.cu"]
-HEADERS = ["acb_build.hpp", "acb_comm.hpp", "acb_device.cuh", "acb_ptx.cuh", "../../include/acb200.h", "../../include/acb200_debug.h"]
+HEADERS = ["acb_build.hpp", "acb_plan.hpp", "acb_fingerprint.cuh", "acb_comm.hpp", "acb_device.cuh", "acb_ptx.cuh", "../../include/acb200.h", "../../include/acb200_debug.h"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = [
     *GENCODE, "-lineinfo", "-O3", "-std=c++17",

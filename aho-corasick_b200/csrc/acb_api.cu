@@ -21,6 +21,7 @@
 #include "acb_build.hpp"
 #include "acb_comm.hpp"
 #include "acb_device.cuh"
+#include "acb_plan.hpp"
 
 using acb::DfaDev;
 using acb::HostDfa;
@@ -109,35 +110,10 @@ struct Workspace {
 
 }  // namespace
 
-// Plan of the prefilter engine for one automaton (derived from the tables alone, so it also
-// works for DFAs adopted through acg_dfa_create).
-struct PrefilterPlan {
-  bool supported = false;
-  uint32_t k = 0, kmask = 0, fold = 0, mult = 1, mult3 = 1, shift = 0, log_bits = 0;
-  uint32_t stride = 1;
-  uint32_t key_shift = 8;  // stride 2: first-stage hash = window * (mult3 << key_shift); 5: the key also
-                           // holds the low 3 bits of the window's fourth byte (default; 8 with ACG_EXP_KEY24)
-  bool wide = false;
-  bool brute = false;
-  uint32_t dup_shift = 0;
-  double fill = 0;          // fraction of bitmap bits set (~ candidate rate on random input)
-  uint64_t n_grams = 0;
-  std::vector<uint32_t> bitmap;
-  bool dense = false;  // many fingerprints: the kernel filters survivors through the anchor map
-  // anchor map: (k-byte haystack prefix -> trie state at depth k), open addressing, see DfaDev::amap
-  std::vector<uint64_t> amap;  // low word = key, high word = premultiplied state id (0 = empty)
-  uint32_t amap_log = 0;
-  // byte-set scan (bytescan_kernel): the needles of the reference's start-bytes / rare-bytes prefilter
-  // when it would have picked one (bs_n == 0: fingerprint filter)
-  uint32_t bs_n = 0;
-  uint8_t bs_byte[3] = {0, 0, 0};
-  uint8_t bs_back[3] = {0, 0, 0};
-};
-
 struct acg_dfa {
   HostDfa h;
   std::vector<uint16_t> depth16;
-  PrefilterPlan pf;
+  acb::PrefilterPlan pf;
   uint32_t* d_bitmap = nullptr;
   uint2* d_amap = nullptr;
   bool has_empty = false;
@@ -253,32 +229,6 @@ void release_workspace(const acg_dfa* a, Workspace* w) {
   a->ws_cv.notify_one();
 }
 
-int bits_for(uint64_t v) {
-  int b = 0;
-  while (v) { ++b; v >>= 1; }
-  return b;
-}
-
-// second Bloom hash; must match bloom_hash2() in acb_prefilter.cu
-uint32_t bloom_hash2(uint32_t x) {
-  x ^= x >> 16;
-  x *= 0x7feb352du;
-  x ^= x >> 15;
-  x *= 0x846ca68bu;
-  x ^= x >> 16;
-  return x;
-}
-
-// third-level hash; must match bloom_hash3() in acb_prefilter.cu
-uint32_t bloom_hash3(uint32_t x) {
-  x ^= x >> 15;
-  x *= 0x2c1b3c6du;
-  x ^= x >> 12;
-  x *= 0x297a2d39u;
-  x ^= x >> 15;
-  return x;
-}
-
 void derive_metadata(acg_dfa* a) {
   HostDfa& h = a->h;
   a->has_empty = h.min_pattern_len == 0 && !h.pattern_lens.empty();
@@ -317,318 +267,7 @@ void derive_metadata(acg_dfa* a) {
   } else {
     a->depth16 = bfs_depth();
   }
-
-  // ---- prefilter plan ----
-  PrefilterPlan& pf = a->pf;
-  pf = PrefilterPlan{};
-  if (h.pattern_lens.empty() || a->has_empty || h.start_unanchored_id == 0) return;
-  if (h.max_pattern_len >= 0xFFFE || h.min_pattern_len == 0) return;
-  // tie-break layout: (max_len - len) << dup_shift | index among the node's own patterns
-  uint32_t max_dups = 1;
-  for (size_t m = 0; m + 1 < h.match_offsets.size(); ++m) {
-    const uint32_t lo = h.match_offsets[m], hi = h.match_offsets[m + 1];
-    const uint32_t dep = (m + 2 < rows) ? a->depth16[m + 2] : 0xFFFF;
-    uint32_t own = 0;
-    for (uint32_t i = lo; i < hi && h.pattern_lens[h.match_pids[i]] == dep; ++i) ++own;
-    max_dups = std::max(max_dups, own);
-  }
-  pf.dup_shift = uint32_t(bits_for(max_dups - 1));
-  if (bits_for(h.max_pattern_len) + int(pf.dup_shift) > acb::kTieBits) return;
-
-  // k-gram fingerprints: every trie path of length k from the start row, over raw bytes
-  const uint32_t kmax = uint32_t(std::min<uint64_t>(4, h.min_pattern_len));
-  struct Item { uint32_t row; uint32_t gram; };
-  std::vector<std::vector<uint32_t>> grams(kmax + 1);
-  std::vector<std::vector<Item>> level(kmax + 1);  // (row, raw bytes) of every trie path of that length
-  std::vector<Item> cur{{h.start_unanchored_id >> s2, 0u}}, nxt;
-  // deferred dense fill: the table does not exist on the host; the builder's shallow trie edges
-  // (grouped by source row, bytes ascending) are the same transitions "one byte deeper"
-  std::vector<uint32_t> sh_first;  // first shallow edge of a row, +1 (0: none)
-  if (h.fill.valid) {
-    sh_first.assign(rows, 0);
-    for (size_t i = h.fill.shallow.size(); i-- > 0;) sh_first[h.fill.shallow[i].from_row] = uint32_t(i + 1);
-  }
-  for (uint32_t j = 0; j < kmax; ++j) {
-    nxt.clear();
-    for (const Item& it : cur) {
-      if (h.fill.valid) {
-        for (size_t i = sh_first[it.row]; i != 0 && i <= h.fill.shallow.size() && h.fill.shallow[i - 1].from_row == it.row; ++i) {
-          const auto& e = h.fill.shallow[i - 1];
-          if (e.to_row == 0 || a->depth16[e.to_row] != j + 1) continue;
-          nxt.push_back(Item{e.to_row, it.gram | (e.byte << (8 * j))});
-        }
-        continue;
-      }
-      const uint32_t* row = h.trans.data() + (size_t(it.row) << s2);
-      for (uint32_t b = 0; b < 256; ++b) {
-        const uint32_t nr = row[h.classes[b]] >> s2;
-        if (nr == 0 || a->depth16[nr] != j + 1) continue;
-        nxt.push_back(Item{nr, it.gram | (b << (8 * j))});
-      }
-    }
-    cur.swap(nxt);
-    level[j + 1] = cur;
-    auto& g = grams[j + 1];
-    g.reserve(cur.size());
-    for (const Item& it : cur) g.push_back(it.gram);
-    std::sort(g.begin(), g.end());
-    g.erase(std::unique(g.begin(), g.end()), g.end());
-    if (cur.size() > (64u << 20)) break;  // pathological fan-out: give up on longer fingerprints
-  }
-  // pick the fingerprint length with the sparsest bitmap (ties -> longer)
-  double best_fill = 2.0;
-  std::vector<uint32_t> best_set;
-  for (uint32_t k = 1; k <= kmax; ++k) {
-    if (grams[k].empty()) continue;
-    std::vector<uint32_t> raw = grams[k], folded = grams[k];
-    for (uint32_t& g : folded) g |= 0x20202020u & (k == 4 ? 0xFFFFFFFFu : ((1u << (8 * k)) - 1));
-    std::sort(folded.begin(), folded.end());
-    folded.erase(std::unique(folded.begin(), folded.end()), folded.end());
-    const bool use_fold = folded.size() * 3 < raw.size() * 2;
-    const std::vector<uint32_t>& set = use_fold ? folded : raw;
-    // Bloom bitmap with two hashes (a single multiply for the per-position probe, a full mix
-    // for the second probe that only first-probe hits pay for).  Bit position of a hash h: byte
-    // from the top (log_bits-3) bits, bit inside the byte from the low 3 bits (little-endian words).
-    // the kernel's bitmap size is a compile-time constant (kBloomLogBits in acb_prefilter.cu)
-    const uint32_t log_bits = 20;
-    const uint32_t mult = 0x9E3779B1u;
-    const uint32_t shift = 35 - log_bits;
-    const uint32_t kmask = k == 4 ? 0xFFFFFFFFu : ((1u << (8 * k)) - 1);
-    std::vector<uint32_t> bm(size_t(1) << (log_bits - 5), 0u);
-    uint64_t set_bits = 0;
-    auto set_hash = [&](uint32_t hsh) {  // byte (hsh >> shift), bit (hsh & 7); see bloom_test()
-      const uint32_t byte = hsh >> shift, bit = byte * 8 + (hsh & 7);
-      uint32_t& wd = bm[bit >> 5];
-      if (!(wd >> (bit & 31) & 1)) { wd |= 1u << (bit & 31); ++set_bits; }
-    };
-    for (uint32_t g : set) {
-      set_hash((g & kmask) * mult);
-      set_hash(bloom_hash2(g & kmask));
-    }
-    double fill = double(set_bits) / double(uint64_t(1) << log_bits);
-    fill = fill * fill;  // both probes must hit
-    // expected candidate rate on text drawn from the patterns' own alphabet: Bloom false positives
-    // plus genuine k-gram prefix hits (n_grams / prod_j |bytes seen at position j|)
-    double space = 1.0;
-    for (uint32_t j = 0; j < k; ++j) {
-      bool seen[256] = {false};
-      unsigned distinct = 0;
-      for (uint32_t g : set) { const uint32_t b = (g >> (8 * j)) & 0xFF; if (!seen[b]) { seen[b] = true; ++distinct; } }
-      space *= double(std::max(distinct, 1u));
-    }
-    fill += std::min(1.0, double(set.size()) / space);
-    if (fill <= best_fill) {
-      best_fill = fill;
-      pf.k = k; pf.kmask = kmask; pf.fold = use_fold ? (0x20202020u & kmask) : 0u;
-      pf.mult = mult; pf.shift = shift; pf.log_bits = log_bits;
-      pf.fill = fill; pf.n_grams = set.size();
-      pf.bitmap.swap(bm);
-      best_set = set;
-      for (uint32_t& g : best_set) g &= kmask;
-    }
-  }
-  if (pf.k == 0) return;
-  // Dense sets (more fingerprints than a two-probe Bloom filter of 2^20 bits can keep apart; cfg 5:
-  // 10^5): a blocked filter instead -- every fingerprint owns one 32-bit word (top 15 bits of
-  // gram * mult) and two bits inside it (bits 0-4 and 5-9 of the product's high half), so that the
-  // per-position probe settles both with a single shared-memory load; the second stage is then the
-  // exact anchor-map lookup.  Must match the DENSE branch of ACB_PROBE in acb_prefilter.cu.
-  const bool dense = best_set.size() > 8192;
-  if (dense) {
-    std::fill(pf.bitmap.begin(), pf.bitmap.end(), 0u);
-    const uint32_t word_shift = 32 - (pf.log_bits - 5);
-    for (uint32_t g : best_set) {
-      const uint64_t prod = uint64_t(g) * pf.mult;
-      const uint32_t lo = uint32_t(prod), hi = uint32_t(prod >> 32);
-      pf.bitmap[lo >> word_shift] |= (1u << (hi & 31)) | (1u << ((hi >> 5) & 31));
-    }
-    // pass rate on text drawn from the bytes the patterns use at each fingerprint position
-    std::vector<uint8_t> alpha[4];
-    for (uint32_t j = 0; j < pf.k; ++j) {
-      bool seen[256] = {false};
-      for (uint32_t g : best_set) seen[(g >> (8 * j)) & 0xFF] = true;
-      for (uint32_t b = 0; b < 256; ++b) if (seen[b]) alpha[j].push_back(uint8_t(b));
-    }
-    uint64_t pass = 0, x = 0x9E3779B97F4A7C15ull;
-    const int kTrials = 65536;
-    for (int i = 0; i < kTrials; ++i) {
-      uint32_t g = 0;
-      for (uint32_t j = 0; j < pf.k; ++j) {
-        x = x * 6364136223846793005ull + 1442695040888963407ull;
-        g |= uint32_t(alpha[j][(x >> 33) % alpha[j].size()]) << (8 * j);
-      }
-      const uint64_t prod = uint64_t(g) * pf.mult;
-      const uint32_t lo = uint32_t(prod), hi = uint32_t(prod >> 32);
-      const uint32_t w = pf.bitmap[lo >> word_shift];
-      pass += (w >> (hi & 31)) & (w >> ((hi >> 5) & 31)) & 1u;
-    }
-    pf.fill = double(pass) / kTrials;
-  }
-  pf.brute = pf.fill > 0.25;
-  pf.supported = true;
-  // Stride-2 first stage: with 4-byte fingerprints and patterns of at least 4 bytes, probing only
-  // every other offset with the 3-byte fingerprints of pattern bytes [0,3) and [1,4) still sees
-  // every occurrence (a pattern that starts at an odd offset shows its second fingerprint at the
-  // next even one) and halves the per-position probe work.  Worth it while those 3-grams stay rare.
-  if (!pf.brute && pf.k == 4 && best_set.size() <= 8192) {
-    const std::vector<Item>& paths4 = level[4];
-    std::vector<uint32_t> g3;
-    g3.reserve(best_set.size() * 2);
-    const uint32_t f3 = pf.fold & 0x00FFFFFFu;
-    for (uint32_t g : best_set) {
-      g3.push_back((g & 0x00FFFFFFu) | f3);
-      g3.push_back((g >> 8) | f3);
-    }
-    std::sort(g3.begin(), g3.end());
-    g3.erase(std::unique(g3.begin(), g3.end()), g3.end());
-    double space = 1.0;
-    for (uint32_t j = 0; j < 3; ++j) {
-      bool seen[256] = {false};
-      unsigned distinct = 0;
-      for (uint32_t g : g3) { const uint32_t b = (g >> (8 * j)) & 0xFF; if (!seen[b]) { seen[b] = true; ++distinct; } }
-      space *= double(std::max(distinct, 1u));
-    }
-    const double n_bits_set = double(g3.size()) + 2.0 * double(best_set.size());
-    const double true3 = double(g3.size()) / space;
-    const double pass1 = n_bits_set / double(uint64_t(1) << pf.log_bits) + true3;  // per probed offset
-    if (pass1 < 0.07) {  // beyond that the second stage costs more than the halved probe count saves
-      pf.stride = 2;
-      // rare hits even with a 16 KiB bitmap: the wide geometry (2 KiB tiles, two CTAs per SM,
-      // PfBloom<true> in acb_prefilter.cu) amortises the per-step bookkeeping better
-      constexpr uint32_t kWideLogBits = 17;
-      pf.wide = n_bits_set / double(uint64_t(1) << kWideLogBits) + true3 < 0.01;
-      if (pf.wide) {
-        pf.log_bits = kWideLogBits;
-        pf.shift = 35 - kWideLogBits;
-        pf.bitmap.assign(size_t(1) << (kWideLogBits - 5), 0u);
-        auto set_hash = [&](uint32_t hsh) {
-          const uint32_t bit = (hsh >> pf.shift) * 8 + (hsh & 7);
-          pf.bitmap[bit >> 5] |= 1u << (bit & 31);
-        };
-        for (uint32_t g : best_set) {
-          set_hash(g * pf.mult);
-          set_hash(bloom_hash2(g));
-        }
-      }
-      // First-stage probe of the stride-2 kernel: byte index from the 3-byte fingerprint times
-      // (mult3 << 8) -- the shifted multiplier discards the fourth window byte -- and the bit inside
-      // the byte from the fingerprint's own low bits.  A multiplicative hash of such short keys is
-      // sensitive to the constant, so pick the candidate that lets through the fewest fingerprints
-      // drawn from the bytes the patterns use at each position.
-      // First-stage keys.  ACG_EXP_KEY24: the 3-byte fingerprints.  Default (faster on cfg 2 and cfg 3): 27-bit keys
-      // -- the 3 bytes plus the low 3 bits of the window's fourth byte, which a shift of 5 instead
-      // of 8 in the multiplier keeps at no cost in the kernel.  For a pattern that starts at the
-      // probed (even) offset the fourth byte is its own fourth byte; for one that starts one byte
-      // earlier it is the pattern's fifth byte -- any of the 8 values if the pattern ends after four
-      // bytes.  Genuine 3-byte prefix hits (the bulk of the first-stage hits of cfg 2) drop 8-fold.
-      const bool key27 = (a->experiment & ACG_EXP_KEY24) == 0;
-      pf.key_shift = key27 ? 5 : 8;
-      std::vector<uint32_t> keys1;
-      if (!key27) {
-        keys1 = g3;
-      } else {
-        for (const Item& it : paths4) {
-          const uint32_t g = it.gram;
-          keys1.push_back(((g & 0x00FFFFFFu) | f3) | (((g >> 24) & 7u) << 24));
-          uint32_t xs = 0;  // bit x: some pattern through this 4-gram continues with a byte whose low bits are x
-          if (it.row >= 2 && (it.row << s2) <= h.max_match_id) {
-            const uint32_t lo = h.match_offsets[it.row - 2], hi = h.match_offsets[it.row - 1];
-            if (lo < hi && h.pattern_lens[h.match_pids[lo]] == 4) xs = 0xFF;  // a 4-byte pattern ends here
-          }
-          if (xs != 0xFF) {
-            if (h.fill.valid) {
-              for (size_t i = sh_first[it.row]; i != 0 && i <= h.fill.shallow.size() && h.fill.shallow[i - 1].from_row == it.row; ++i)
-                if (a->depth16[h.fill.shallow[i - 1].to_row] == 5) xs |= 1u << (h.fill.shallow[i - 1].byte & 7);
-            } else {
-              const uint32_t* row = h.trans.data() + (size_t(it.row) << s2);
-              for (uint32_t b = 0; b < 256; ++b) {
-                const uint32_t nr = row[h.classes[b]] >> s2;
-                if (nr != 0 && a->depth16[nr] == 5) xs |= 1u << (b & 7);
-              }
-            }
-          }
-          for (uint32_t x = 0; x < 8; ++x)
-            if (xs >> x & 1) keys1.push_back(((g >> 8) | f3) | (x << 24));
-        }
-        std::sort(keys1.begin(), keys1.end());
-        keys1.erase(std::unique(keys1.begin(), keys1.end()), keys1.end());
-      }
-      static const uint32_t kCand[] = {0x1B873593u, 0x27D4EB2Fu, 0x165667B1u, 0x9E3779B1u, 0x2C1B3C6Du,
-                                       0xB5297A4Du, 0x85EBCA6Bu, 0x5BD1E995u, 0x7FEB352Du, 0xCC9E2D51u,
-                                       0x1B56C4E9u, 0xC2B2AE35u};
-      std::vector<uint8_t> alpha[3];
-      for (uint32_t j = 0; j < 3; ++j) {
-        bool seen[256] = {false};
-        for (uint32_t g : g3) seen[(g >> (8 * j)) & 0xFF] = true;
-        for (uint32_t b = 0; b < 256; ++b) if (seen[b]) alpha[j].push_back(uint8_t(b));
-      }
-      const uint32_t ks = pf.key_shift;
-      auto bit_of = [&](uint32_t g, uint32_t m) -> uint32_t {
-        return ((g * (m << ks)) >> pf.shift) * 8 + (g & 7);
-      };
-      uint32_t best_m = kCand[0];
-      uint64_t best_pass = UINT64_MAX;
-      std::vector<uint32_t> trial;
-      for (uint32_t m : kCand) {
-        trial = pf.bitmap;
-        for (uint32_t g : keys1) { const uint32_t bit = bit_of(g, m); trial[bit >> 5] |= 1u << (bit & 31); }
-        uint64_t pass = 0, x = 0x9E3779B97F4A7C15ull;
-        for (int i = 0; i < 65536; ++i) {
-          x = x * 6364136223846793005ull + 1442695040888963407ull;
-          const uint32_t r = uint32_t(x >> 33);
-          uint32_t g = uint32_t(alpha[0][r % alpha[0].size()]) |
-                       uint32_t(alpha[1][(r >> 10) % alpha[1].size()]) << 8 |
-                       uint32_t(alpha[2][(r >> 20) % alpha[2].size()]) << 16;
-          if (key27) g |= uint32_t((x >> 20) & 7) << 24;
-          const uint32_t bit = bit_of(g, m);
-          pass += (trial[bit >> 5] >> (bit & 31)) & 1u;
-        }
-        if (pass < best_pass) { best_pass = pass; best_m = m; }
-      }
-      pf.mult3 = best_m;
-      for (uint32_t g : keys1) {
-        const uint32_t bit = bit_of(g, best_m);
-        pf.bitmap[bit >> 5] |= 1u << (bit & 31);
-      }
-    }
-  }
-  pf.dense = !pf.brute && dense;
-  // Anchor map: the verifier looks the first k bytes at a candidate offset up here and starts at
-  // depth k.  Keys are raw (unfolded) byte strings: one entry per trie path of length k.
-  const std::vector<Item>& paths = level[pf.k];
-  if (!paths.empty() && paths.size() <= (4u << 20)) {
-    // load factor <= 1/4: a lookup of a key that is not there (the common case) ends at the first slot
-    // three times out of four, and every further slot is another dependent L2 access
-    pf.amap_log = uint32_t(std::max(4, bits_for(uint64_t(paths.size()) * 4 - 1)));
-    pf.amap.assign(size_t(1) << pf.amap_log, 0ull);
-    const uint32_t cap_mask = (1u << pf.amap_log) - 1;
-    for (const Item& it : paths) {
-      const uint32_t key = it.gram & pf.kmask;
-      uint32_t slot = bloom_hash3(key) >> (32 - pf.amap_log);
-      while (pf.amap[slot] != 0 && uint32_t(pf.amap[slot]) != key) slot = (slot + 1) & cap_mask;
-      pf.amap[slot] = uint64_t(key) | (uint64_t(it.row << s2) << 32);
-    }
-  }
-  // Byte-set scan for the automata the reference gives a start-bytes / rare-bytes prefilter
-  // (src/util/prefilter.rs:163-305).  Tables built here carry the set; for an adopted table that
-  // reports start bytes the set is read off the start row (the first bytes of all patterns).
-  if (h.prefilter_kind == ACG_PRE_START_BYTES || h.prefilter_kind == ACG_PRE_RARE_BYTES) {
-    if (h.pre_n) {
-      // Needles with offsets (rare bytes in the middle of patterns) turn every occurrence into
-      // back + 1 start offsets to verify; on BASELINE config 1's automaton over uniform printable text
-      // that is slower than the fingerprint filter, so the scan is reserved for needles that mark a
-      // pattern's first byte.
-      bool ok = true;
-      for (uint32_t i = 0; i < h.pre_n; ++i) ok = ok && h.pre_back[i] == 0;
-      if (ok) {
-        pf.bs_n = h.pre_n;
-        for (uint32_t i = 0; i < h.pre_n; ++i) { pf.bs_byte[i] = h.pre_byte[i]; pf.bs_back[i] = h.pre_back[i]; }
-      }
-    } else if (h.prefilter_kind == ACG_PRE_START_BYTES && !level[1].empty() && grams[1].size() <= 3) {
-      pf.bs_n = uint32_t(grams[1].size());
-      for (uint32_t i = 0; i < pf.bs_n; ++i) { pf.bs_byte[i] = uint8_t(grams[1][i]); pf.bs_back[i] = 0; }
-    }
-  }
+  a->pf = acb::plan_prefilter(h, a->depth16, (a->experiment & ACG_EXP_KEY24) != 0);
 }
 
 // Dense table produced on the device from the builder's DenseFillPlan (acb_build.hpp): one
@@ -729,10 +368,7 @@ int upload(acg_dfa* a) {
   d.max_pattern_len = uint32_t(std::min<uint64_t>(h.max_pattern_len, UINT32_MAX));
   d.min_pattern_len = uint32_t(std::min<uint64_t>(h.min_pattern_len, UINT32_MAX));
   d.amap = a->d_amap;
-  d.amap_shift = a->pf.amap_log ? 32 - a->pf.amap_log : 0;
-  d.amap_mask = a->pf.amap_log ? (1u << a->pf.amap_log) - 1 : 0;
-  d.amap_k = a->pf.k;
-  d.amap_kmask = a->pf.kmask;
+  acb::plan_device_fields(a->pf, d);
   a->on_device = true;
   return ACG_OK;
 }
@@ -813,7 +449,7 @@ struct BucketPlan {
 BucketPlan plan_buckets(const acg_dfa* a, uint64_t n_bytes) {
   BucketPlan b;
   if (a->experiment & ACG_EXP_GLOBAL_TILES) return b;
-  const uint32_t tie_bits = uint32_t(bits_for(a->h.max_pattern_len)) + a->pf.dup_shift;
+  const uint32_t tie_bits = uint32_t(acb::bit_width(a->h.max_pattern_len)) + a->pf.dup_shift;
   if (tie_bits >= 32) return b;
   const uint32_t max_shift = 32 - tie_bits;
   uint32_t shift = std::min<uint32_t>(25, max_shift);
@@ -842,7 +478,7 @@ int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t rea
                             uint64_t scan_hi, int mode, int dev_sms, const BucketPlan& bp,
                             const DocBatch* docs) {
   Workspace& w = cur_ws();
-  const PrefilterPlan& pf = a->pf;
+  const acb::PrefilterPlan& pf = a->pf;
   // 16-byte aligned filter region whose 4-byte look-ahead stays inside the readable bytes
   const uintptr_t base = reinterpret_cast<uintptr_t>(d_hay);
   uint64_t lo = scan_lo + ((16 - ((base + scan_lo) & 15)) & 15);
@@ -861,7 +497,6 @@ int enqueue_prefilter_range(const acg_dfa* a, const uint8_t* d_hay, uint64_t rea
   p.stride = pf.stride;
   // kernel geometry as planned; second-stage organisation and tile distribution: see prefilter_kernel
   p.geom = pf.wide ? 1 : 0;
-  p.pair = 0;
   p.dyn = (a->experiment & ACG_EXP_STATIC_TILES) ? 0 : ((a->experiment & ACG_EXP_GLOBAL_TILES) ? 2 : 1);
   p.kmask = pf.kmask;
   p.fold = pf.fold;
@@ -912,7 +547,7 @@ int order_tuples(const acg_dfa* a, uint64_t want, uint64_t n_bytes, TupleResult*
   cur_ws().stats.raw_matches = want;
   res->sorted_buf = 0;
   if (want <= 1 && (bp.shift == 0 || want == 0)) return ACG_OK;  // (one bucketed tuple still has to move to slot 0)
-  const int end_bit = std::min(64, acb::kTieBits + bits_for(n_bytes + 1));
+  const int end_bit = std::min(64, acb::kTieBits + acb::bit_width(n_bytes + 1));
   float ms = 0;
   CK(cudaEventRecord(w.ev2, w.stream));
   // the list in buffer `from`, ordered into the other one
@@ -1587,7 +1222,6 @@ int sharded_begin(const acg_dfa* a, acg_comm* c, const uint8_t* hay, bool hay_on
     // blocking step: the kernel stores the records straight into rank 0's buffer.  Stream of steps
     // (begin / wait): it expands into local memory -- short, HBM-bound -- and a copy engine ships the
     // records, so that the next step's scan, which starts right behind, finds every SM free.
-    e.small = 0;
     CK(acb::launch_expand(e, c->stream));
   }
   bool flagged = false;
@@ -2211,7 +1845,7 @@ int acg_packed_variant(const acg_dfa* a, int* fat, int* mask_len) {
 
 int acg_debug_prefilter_plan(const acg_dfa* a, acg_prefilter_plan* out) {
   if (!a || !out) return ACG_E_INVALID_ARG;
-  const PrefilterPlan& pf = a->pf;
+  const acb::PrefilterPlan& pf = a->pf;
   *out = acg_prefilter_plan{};
   out->supported = pf.supported ? 1 : 0;
   out->brute = pf.brute ? 1 : 0;
@@ -2243,7 +1877,7 @@ int acg_debug_set_experiment(acg_dfa* a, uint32_t flags) {
   if (changed & ACG_EXP_KEY24) {
     // the first-stage keys are part of the plan: rebuild it and refresh the device copy of the bitmap
     const size_t old_words = a->pf.bitmap.size();
-    derive_metadata(a);
+    a->pf = acb::plan_prefilter(a->h, a->depth16, (flags & ACG_EXP_KEY24) != 0);
     if (a->on_device && a->d_bitmap && a->pf.supported) {
       if (a->pf.bitmap.size() != old_words) return ACG_E_INVALID_ARG;  // the geometry does not depend on the keys
       DeviceGuard guard(a->device);

@@ -179,7 +179,6 @@ struct PrefilterLaunch {
                                 // 3-byte fingerprints of pattern bytes [0,3) and [1,4) (k == 4 only)
   uint16_t geom;                // stride 2 only: 0 narrow, 1 wide (2 KiB tiles / 512 threads / 16 KiB bitmap: rare
                                 // first-stage hits)
-  uint16_t pair;                // (unused)
   uint32_t kmask;               // mask of the low k bytes
   uint32_t fold;                // 0 or 0x20202020 (ASCII case folding of the fingerprint)
   uint32_t mult;                // first Bloom hash: gram * mult
@@ -248,8 +247,6 @@ struct ExpandLaunch {
   uint64_t span_start;
   uint64_t offset_add;
   uint64_t* out;         // [ (n-first) * 3 ] as (pid, start, end) u64 triples == acg_match layout
-  int small = 0;         // > 0: that many 128-thread CTAs at most (one per SM: each fits beside a persistent scan
-                         // CTA, pipelined sharded steps); 0: one 256-thread CTA per 256 records
 };
 cudaError_t launch_expand(const ExpandLaunch& e, cudaStream_t s);
 // number of leading tuples whose end_rel <= bound (keys sorted ascending)

@@ -384,14 +384,12 @@ __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint
 
 // Records built in shared memory and stored as 16-byte vectors: the target may be another GPU's HBM
 // (peer mapping of rank 0's receive buffer, acb_comm.hpp), where full lines per warp store matter
-// more than at home.  Two sizes: 256 records per CTA, and a small one -- 128 threads, 3 KB of shared
-// memory -- that fits beside the persistent scan CTA of the next sharded step on the same SM, so that
-// the transfer overlaps that scan.  Record = acg_match { u32 pid; u32 pad; u64 start; u64 end }.
-template <int kExpandThreads>
+// more than at home.  256 records per CTA.  Record = acg_match { u32 pid; u32 pad; u64 start; u64 end }.
+constexpr int kExpandThreads = 256;
 __global__ void __launch_bounds__(kExpandThreads) expand_kernel(ExpandLaunch e) {
   __shared__ uint64_t s_rec[kExpandThreads * 3];
   const uint64_t m = e.t.n - e.first;
-  // grid-stride over blocks of kExpandThreads records (the small form runs one CTA per SM)
+  // grid-stride over blocks of kExpandThreads records
   for (uint64_t base = (uint64_t)blockIdx.x * kExpandThreads; base < m; base += (uint64_t)gridDim.x * kExpandThreads) {
     const uint64_t i = base + threadIdx.x;
     if (i < m) {
@@ -433,13 +431,7 @@ __global__ void lower_bound_kernel(const uint64_t* keys, uint64_t n, uint64_t bo
 cudaError_t launch_expand(const ExpandLaunch& e, cudaStream_t s) {
   const uint64_t m = e.t.n - e.first;
   if (m == 0) return cudaSuccess;
-  if (e.small) {
-    // one small CTA per SM at most: the persistent scan CTA of the next step must still fit beside it
-    const uint64_t blocks = (m + 127) / 128;
-    ACB_LAUNCH(expand_kernel<128>, (unsigned)(blocks < (uint64_t)e.small ? blocks : (uint64_t)e.small), 128, 0, s, e);
-  } else {
-    ACB_LAUNCH(expand_kernel<256>, (unsigned)((m + 255) / 256), 256, 0, s, e);
-  }
+  ACB_LAUNCH(expand_kernel, (unsigned)((m + kExpandThreads - 1) / kExpandThreads), kExpandThreads, 0, s, e);
   return cudaGetLastError();
 }
 cudaError_t launch_lower_bound(const uint64_t* keys, uint64_t n, uint64_t bound_key,

@@ -13,6 +13,7 @@
 // (depth(state) == bytes consumed) and reports the node's own patterns -- the set
 // of patterns that are a prefix of the haystack at that offset.
 #include "acb_device.cuh"
+#include "acb_fingerprint.cuh"
 #ifndef ACB_PTX_HEADER
 #define ACB_PTX_HEADER "acb_ptx.cuh"
 #endif
@@ -44,6 +45,9 @@ template <int GEOM> struct PfGeom {
   static constexpr int kTile = kGroups * 512;           // haystack bytes per warp step
   static constexpr int kStageBytes = kTile + 16;        // + fingerprint look-ahead
   static constexpr int kMinCtas = GEOM == kGeomWide ? 2 : 1;
+  // Bloom bitmap size: a compile-time constant, so that the byte index (hash >> shift) and the
+  // shared-memory base fold into one address instruction
+  static constexpr uint32_t kLogBits = GEOM == kGeomWide ? kWideLogBits : kNarrowLogBits;
 };
 // per-warp queue sizes: first-probe hits of one step handled by the compacted second probe, and
 // verified-candidate entries (the dense variant stores 8-byte entries, so fewer of them fit
@@ -52,28 +56,6 @@ template <bool DENSE> struct PfCfg {
   static constexpr int kSlots = 256;
   static constexpr int kQ2 = DENSE ? 64 : 96;
 };
-
-// Second Bloom hash: a full avalanche mix (evaluated only for first-probe hits, so its cost is
-// irrelevant); the first probe is a single multiply.  Must match bloom_hash2() in acb_api.cu.
-__device__ __forceinline__ uint32_t bloom_hash2(uint32_t x) {
-  x ^= x >> 16;
-  x *= 0x7feb352du;
-  x ^= x >> 15;
-  x *= 0x846ca68bu;
-  x ^= x >> 16;
-  return x;
-}
-
-// Third-level fingerprint hash (global-memory bitmap, only for automata with many patterns).
-// Must match bloom_hash3() in acb_api.cu.
-__device__ __forceinline__ uint32_t bloom_hash3(uint32_t x) {
-  x ^= x >> 15;
-  x *= 0x2c1b3c6du;
-  x ^= x >> 12;
-  x *= 0x297a2d39u;
-  x ^= x >> 15;
-  return x;
-}
 
 // Queued offsets are 32-bit, inside a window of 2^kWinShift bytes of the chunk (prefilter_kernel).
 // The dry run can shrink the window (ACB_EMU_WINSHIFT) so that small inputs cross many of them.
@@ -144,8 +126,18 @@ struct Emitter {
   }
 };
 
-// Anchor-map lookup: the state reached from the start state by the k bytes at `s`, 0 if those
-// bytes are not the beginning of any pattern.  Must match the table built in acb_api.cu.
+// Anchor-map lookup (acb_fingerprint.cuh): the state reached from the start state by `key`, the raw
+// first k bytes at an offset; 0 if those bytes are not the beginning of any pattern.
+__device__ __forceinline__ uint32_t anchor_lookup_key(const DfaDev& d, uint32_t key) {
+  uint32_t slot = amap_slot(key, d.amap_shift);
+  for (;;) {
+    const uint2 e = __ldg(d.amap + slot);
+    if (e.y == 0 || e.x == key) return e.y;
+    slot = amap_next(slot, d.amap_mask);
+  }
+}
+
+// The same lookup for the k bytes at haystack offset `s`.
 __device__ __forceinline__ uint32_t anchor_lookup(const DfaDev& d, const PrefilterLaunch& p, uint64_t s) {
   if (s + d.amap_k > p.span_end) return 0;  // no pattern fits any more
   // the k bytes at s: two aligned word loads when both words lie inside the haystack buffer,
@@ -163,23 +155,7 @@ __device__ __forceinline__ uint32_t anchor_lookup(const DfaDev& d, const Prefilt
     key = 0;
     for (uint32_t i = 0; i < d.amap_k; ++i) key |= (uint32_t)__ldg(p.hay + s + i) << (8 * i);
   }
-  uint32_t slot = bloom_hash3(key) >> d.amap_shift;
-  for (;;) {
-    const uint2 e = __ldg(d.amap + slot);
-    if (e.y == 0 || e.x == key) return e.y;
-    slot = (slot + 1) & d.amap_mask;
-  }
-}
-
-// The same lookup for a key already in a register (the dense variant's second stage reads the
-// candidate's bytes out of the staged tile): `key` = the raw first k bytes at the offset.
-__device__ __forceinline__ uint32_t anchor_lookup_key(const DfaDev& d, uint32_t key) {
-  uint32_t slot = bloom_hash3(key) >> d.amap_shift;
-  for (;;) {
-    const uint2 e = __ldg(d.amap + slot);
-    if (e.y == 0 || e.x == key) return e.y;
-    slot = (slot + 1) & d.amap_mask;
-  }
+  return anchor_lookup_key(d, key);
 }
 
 // Batched search: the end of the document that contains start offset s, i.e. doc_offsets[i] for the
@@ -254,21 +230,11 @@ __device__ __forceinline__ void verify_at(const DfaDev& d, const PrefilterLaunch
   }
 }
 
-// The size of the shared-memory Bloom bitmap is a compile-time property of the kernel geometry,
-// so that the byte index (hash >> shift) and the shared-memory base fold into one address
-// instruction: 2^20 bits (128 KiB) in general; 2^17 bits (16 KiB) for the wide geometry, which is
-// only chosen for small pattern sets and then leaves room for two CTAs per SM.
-template <int GEOM> struct PfBloom {
-  static constexpr uint32_t kLogBits = GEOM == kGeomWide ? 17 : 20;
-  static constexpr uint32_t kShift = 35 - kLogBits;
-};
-
-// Bit position of a 32-bit hash in the Bloom bitmap: the byte comes from the top (log_bits-3)
+// Bloom probe of a 32-bit hash, bloom_bit(h, h, SHIFT): the byte comes from the top (log_bits-3)
 // bits, the bit inside the byte from the low 3 bits.  The probe loads that byte, replicates it
 // into all four byte lanes with a multiply (FMA pipe) and rotates by the raw hash (the hardware
 // uses the shift amount mod 32), which puts bit (h & 7) of the byte at bit 0 -- one shift, one
-// byte load, one multiply and one rotate per position, no masking.  Must match set_hash() in
-// acb_api.cu.
+// byte load, one multiply and one rotate per position, no masking.
 template <uint32_t SHIFT>
 __device__ __forceinline__ bool bloom_test(const uint32_t* s_bitmap, uint32_t h) {
   const uint32_t byte = reinterpret_cast<const uint8_t*>(s_bitmap)[h >> SHIFT];
@@ -317,9 +283,8 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   constexpr int kPfStageBytes = kPfTile + 16;  // + fingerprint look-ahead
   constexpr int kGroups = PfPass<GEOM, STRIDE>::kGroups;
   constexpr int kPfSlots = PfCfg<DENSE>::kSlots;
-  constexpr int kSlotsAlloc = kPfSlots;
   constexpr int kPfQ2 = PfCfg<ANCH>::kQ2;
-  constexpr uint32_t kBloomShift = PfBloom<GEOM>::kShift;
+  constexpr uint32_t kBloomShift = bloom_shift(PfGeom<GEOM>::kLogBits);
   using Q2Entry = typename std::conditional<ANCH, uint2, uint32_t>::type;  // (offset[, trie state of its first k bytes])
   ACB_DYNAMIC_SMEM(smem_raw);
   unsigned char* s_ring = smem_raw;                                    // [kPfWarps][kRingBytes]
@@ -327,8 +292,8 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   uint32_t* s_tile_of = reinterpret_cast<uint32_t*>(s_bars + kPfWarps * kPfStages);  // DYN: tile number staged in [warp][stage]
   uint32_t* s_next_tile = s_tile_of + kPfWarps * kPfStages;                        // DYN: draw state (u64), prefetched super-tile (u32), pad
   Q2Entry* s_queue2 = reinterpret_cast<Q2Entry*>(s_next_tile + 4);  // [kPfWarps][kPfQ2]
-  uint16_t* s_slots = reinterpret_cast<uint16_t*>(s_queue2 + kPfWarps * kPfQ2);  // [kPfWarps][kSlotsAlloc]
-  uint32_t* s_bitmap = reinterpret_cast<uint32_t*>(s_slots + kPfWarps * kSlotsAlloc);
+  uint16_t* s_slots = reinterpret_cast<uint16_t*>(s_queue2 + kPfWarps * kPfQ2);  // [kPfWarps][kPfSlots]
+  uint32_t* s_bitmap = reinterpret_cast<uint32_t*>(s_slots + kPfWarps * kPfSlots);
   __shared__ uint8_t s_cls[256];
 
   const int tid = threadIdx.x;
@@ -387,9 +352,9 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
 
   const uint32_t kmask = p.kmask, fold = p.fold, mult = p.mult;
   const uint32_t fold1 = p.fold & 0x00FFFFFFu;  // stride 2: the first stage fingerprints 3 bytes
-  // stride 2: multiplying by (mult << 8) drops the window's fourth byte for free; the bit inside
+  // stride 2: multiplying by (mult3 << 8) drops the window's fourth byte for free; the bit inside
   // the bitmap byte then comes from the fingerprint's own low bits (the product's are zero)
-  const uint32_t mult8 = p.mult3 << p.key_shift;  // 8: 24-bit keys; 5: 27-bit keys (experiment)
+  const uint32_t mult8 = key_mult(p.mult3, p.key_shift);  // 8: 24-bit keys; 5: 27-bit keys (default)
   // queue offsets are relative to chunk_base: a stride-2 probe at the first byte of the chunk
   // also owns the start one byte before it
   // (unsigned arithmetic: for chunk_lo == 0 the base wraps to 2^64 - 1 and base + rel, rel >= 1, is the
@@ -399,7 +364,7 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
   const uint8_t* s_bytes = reinterpret_cast<const uint8_t*>(s_bitmap);
   unsigned char* ring = s_ring + warp * kRingBytes;
   uint64_t* bars = s_bars + warp * kPfStages;
-  uint16_t* slots = s_slots + warp * kSlotsAlloc;
+  uint16_t* slots = s_slots + warp * kPfSlots;
   Q2Entry* q2 = s_queue2 + warp * kPfQ2;
   uint32_t q2len = 0;  // warp-uniform
   // queued offsets are 32-bit, relative to chunk_base + (q2win << kWinShift): a warp's tiles only
@@ -597,9 +562,10 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
     }                                                                                         \
     if constexpr (DENSE) {                                                                    \
       /* blocked filter: one word per key (top bits of the product), two bits inside it (low    \
-         bits of the product's high half) -- both tested with this one load */                  \
+         bits of the product's high half) -- both tested with this one load; the rotates take    \
+         their amounts mod 32, which are the bits dense_bit_a(ph) and dense_bit_b(ph) */         \
       const uint32_t ph = __umulhi(gm, mult);                                                  \
-      const uint32_t bw = s_bitmap[h >> (kBloomShift + 2)];                                    \
+      const uint32_t bw = s_bitmap[dense_word(h, kBloomShift)];                                \
       mask = __funnelshift_r(mask, __funnelshift_r(bw, bw, ph) & __funnelshift_r(bw, bw, ph >> 5), 1); \
     } else {                                                                                  \
       const uint32_t rep = (uint32_t)s_bytes[h >> kBloomShift] * 0x01010101u;                 \
@@ -641,9 +607,8 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
     const uint32_t lt = (1u << lane) - 1;
     constexpr int kPlanes = DENSE ? 4 : 3;  // per-lane hit counts the ballot prefix sum covers (dense: 32 probes per lane)
     uint32_t slot = 0, total = 0;
-    constexpr int kSumPlanes = kPlanes;
 #pragma unroll
-    for (int b = 0; b < kSumPlanes; ++b) {
+    for (int b = 0; b < kPlanes; ++b) {
       const uint32_t bl = __ballot_sync(0xffffffffu, (cnt >> b) & 1u);
       slot += __popc(bl & lt) << b;
       total += __popc(bl) << b;
@@ -708,7 +673,7 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
                   const uint32_t off = e - j;
                   const uint32_t sa = tile_a + (off & ~3u);
                   key2[u] = __funnelshift_r(ptx::lds32(sa), ptx::lds32(sa + 4), (off & 3) * 8) & d.amap_kmask;
-                  slot2[u] = bloom_hash3(key2[u]) >> d.amap_shift;
+                  slot2[u] = amap_slot(key2[u], d.amap_shift);
                   look[u] = true;
                 }
               }
@@ -720,7 +685,7 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
             for (int u = 0; u < 2; ++u) {
               if (look[u]) {
                 while (ent[u].y != 0 && ent[u].x != key2[u]) {  // open addressing, empty slot = miss
-                  slot2[u] = (slot2[u] + 1) & d.amap_mask;
+                  slot2[u] = amap_next(slot2[u], d.amap_mask);
                   ent[u] = __ldg(d.amap + slot2[u]);
                 }
                 sid2[u] = ent[u].y;
@@ -739,7 +704,7 @@ prefilter_kernel(DfaDev d, PrefilterLaunch p) {
           const uint32_t w = base + lane;
           const uint32_t j = STRIDE == 2 ? (w & 1u) : 0u;
           bool pass = false;
-          uint32_t gram_keep = 0, e = 0;
+          uint32_t e = 0;
           if (w < n_items) {
             const uint32_t raw = slots[STRIDE == 2 ? (w >> 1) : w];
             e = hit_offset(raw & 31u, raw >> 5);
@@ -1156,8 +1121,8 @@ cudaError_t launch_prefilter(const DfaDev& dfa, const PrefilterLaunch& p, int sm
   const bool dense = p.dense != 0;
   const int geom = p.stride == 2 ? p.geom : kGeomNarrow;
   if (geom < kGeomNarrow || geom > kGeomWide) return cudaErrorInvalidValue;
-  const uint32_t want_log = geom == kGeomWide ? PfBloom<kGeomWide>::kLogBits : PfBloom<kGeomNarrow>::kLogBits;
-  if (!p.brute && (p.log_bits != want_log || p.shift != 35 - want_log)) return cudaErrorInvalidValue;
+  const uint32_t want_log = geom == kGeomWide ? PfGeom<kGeomWide>::kLogBits : PfGeom<kGeomNarrow>::kLogBits;
+  if (!p.brute && (p.log_bits != want_log || p.shift != bloom_shift(want_log))) return cudaErrorInvalidValue;
   const size_t bitmap_bytes = p.brute ? 0 : (size_t(1) << (p.log_bits - 3));
   static const int kThreadsOf[2] = {PfGeom<0>::kThreads, PfGeom<1>::kThreads};
   static const int kStageOf[2] = {PfGeom<0>::kStageBytes, PfGeom<1>::kStageBytes};

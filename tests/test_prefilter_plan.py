@@ -1,11 +1,12 @@
 """CPU checks of the device engine's derived tables (include/acb200_debug.h).
 
-The kernels in csrc/acb_prefilter.cu and the host code in csrc/acb_api.cu share a contract: how a
-fingerprint is hashed into the shared-memory Bloom bitmap and how the anchor map is probed.  The
-probe functions are restated here (they are a handful of integer operations) and checked against
-the tables the library builds -- no false negatives for any pattern beginning, and the anchor map
-must agree with a walk of the DFA table (which itself is bit-identical to the oracle's,
-tests/test_product_host.py).  Runs without a GPU on host-only handles.
+The kernels in csrc/acb_prefilter.cu and the plan built by csrc/acb_plan.hpp share a contract, written
+down once in csrc/acb_fingerprint.cuh: how a fingerprint is hashed into the shared-memory Bloom bitmap
+and how the anchor map is probed.  The probe functions are restated here independently (they are a
+handful of integer operations) and checked against the tables the library builds -- no false
+negatives for any pattern beginning, and the anchor map must agree with a walk of the DFA table
+(which itself is bit-identical to the oracle's, tests/test_product_host.py).  Runs without a GPU on
+host-only handles.
 """
 import ctypes as C
 import random
@@ -41,7 +42,7 @@ def plan_of(ac):
     return p
 
 
-def hash2(x):  # bloom_hash2 in acb_prefilter.cu / acb_api.cu
+def hash2(x):  # bloom_hash2 in acb_fingerprint.cuh
     x ^= x >> 16
     x = (x * 0x7FEB352D) & M32
     x ^= x >> 15
