@@ -159,6 +159,10 @@ def _declare(lib):
     lib.acg_find_overlapping_batch_devout.argtypes = lib.acg_find_iter_batch_devout.argtypes
     lib.acg_is_match_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _vp]
     lib.acg_find_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _i, _vp, _vp]
+    lib.acg_pattern_counts_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _i, _vp, _vp, _vp, _u64,
+                                             C.POINTER(_u64)]
+    lib.acg_pattern_counts_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _i, _vp, _vp, _vp, _u64,
+                                                    C.POINTER(_u64)]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -865,6 +869,67 @@ class AhoCorasick:
         if rc:
             self._raise(rc)
         return found, records
+
+    # ---- pattern counts per document (acg_pattern_counts_batch) ----
+    # How often each pattern occurs in each document: the records of find_overlapping_iter_batch (overlapping) or
+    # find_iter_batch, counted by (document, pattern) on the device, as a CSR matrix [n_docs x patterns_len()].
+    def _counts_until_it_fits(self, alloc, call):
+        """The two-call overflow protocol for the (pids, counts) arrays: returns (pids, counts) cut to nnz."""
+        cnt = _u64()
+        cap = self._cap_hint
+        while True:
+            pids, counts = alloc(cap)
+            rc = call(pids, counts, cap, C.byref(cnt))
+            if rc == E_OVERFLOW:
+                cap = int(cnt.value) + int(cnt.value) // 8 + 64
+                self._cap_hint = max(self._cap_hint, cap)
+                continue
+            if rc:
+                self._raise(rc)
+            return pids[: cnt.value], counts[: cnt.value]
+
+    def pattern_counts_batch_np(self, docs, overlapping=False, anchored=Anchored.No):
+        """(row_offsets uint64 [n_docs + 1], pids uint32 [nnz], counts uint64 [nnz]): document d's patterns are
+        pids[row_offsets[d]:row_offsets[d + 1]], ascending, each occurring counts[i] times in it.  `docs` as in
+        find_iter_batch_np."""
+        keep, ptr, n, on_dev, offs = _batch_input(docs)
+        n_docs = offs.size - 1
+        rows = np.empty(n_docs + 1, dtype=np.uint64)
+        pids, counts = self._counts_until_it_fits(
+            lambda cap: (np.empty(cap, np.uint32), np.empty(cap, np.uint64)),
+            lambda pids, counts, cap, nnz: _lib.acg_pattern_counts_batch(
+                self._h, ptr, on_dev, n, offs.ctypes.data, n_docs, int(anchored), int(overlapping), rows.ctypes.data,
+                pids.ctypes.data, counts.ctypes.data, cap, nnz))
+        return rows, pids, counts
+
+    def pattern_counts_batch_devout(self, d_hay_ptr, hay_len, offsets, row_offsets_ptr, pids_ptr, counts_ptr, cap,
+                                    overlapping=False, anchored=Anchored.No, n_docs=None):
+        """The counts into device memory: row_offsets_ptr [n_docs + 1] uint64, pids_ptr [cap] uint32, counts_ptr
+        [cap] uint64.  Returns nnz; raises OverflowError(needed) if cap is too small (nothing is written then)."""
+        keep, optr, n_docs, on_dev = _devout_offsets(offsets, n_docs)
+        nnz = _u64()
+        rc = _lib.acg_pattern_counts_batch_devout(self._h, d_hay_ptr, hay_len, optr, on_dev, n_docs, int(anchored),
+                                                  int(overlapping), row_offsets_ptr, pids_ptr, counts_ptr, cap,
+                                                  C.byref(nnz))
+        if rc == E_OVERFLOW:
+            raise OverflowError(int(nnz.value))
+        if rc:
+            self._raise(rc)
+        return int(nnz.value)
+
+    def pattern_counts_batch_torch(self, docs, overlapping=False, anchored=Anchored.No):
+        """The counts as a CUDA torch.sparse_csr_tensor of size (n_docs, patterns_len()) on the values' device, with
+        int64 crow / col indices and values.  `docs` as in find_iter_batch_torch."""
+        import torch
+        values, keep, optr, n_docs, on_dev = _torch_batch(docs)
+        dev = values.device
+        rows = torch.empty(n_docs + 1, dtype=torch.int64, device=dev)
+        pids, counts = self._counts_until_it_fits(
+            lambda cap: (torch.empty(cap, dtype=torch.int32, device=dev), torch.empty(cap, dtype=torch.int64, device=dev)),
+            lambda pids, counts, cap, nnz: _lib.acg_pattern_counts_batch_devout(
+                self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs, int(anchored), int(overlapping),
+                rows.data_ptr(), pids.data_ptr(), counts.data_ptr(), cap, nnz))
+        return torch.sparse_csr_tensor(rows, pids.to(torch.int64), counts, size=(n_docs, self.patterns_len()))
 
     # ---- replace / stream: host-side glue over find_iter, as in the reference -------------------
     @staticmethod

@@ -1414,15 +1414,126 @@ struct BatchDevOut {
   uint64_t* match_offsets = nullptr;  // find_iter / overlapping: [n_docs + 1]
 };
 
-// acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch / acg_find_batch (include/acb200.h).
-// is_match and find give one result per document: flags[n_docs] (find: found) and, for find, out[n_docs].
+// acg_pattern_counts_batch(_devout): instead of the records of a find_iter / overlapping batch, how often each
+// pattern occurs in each document, as a CSR matrix (host or device arrays, as the call's other outputs).
+struct BatchCounts {
+  uint64_t* row_offsets;  // [n_docs + 1]
+  uint32_t* pids;         // [cap]
+  uint64_t* counts;       // [cap]
+};
+
+// The n matches of a batch -- the tuples `t` of the prefilter engine, or (t.keys == nullptr) the records the
+// sequential engine left at w.d_rec -- counted by (document, pattern) into `co` (CountKeysLaunch and
+// CountRunsLaunch, acb_device.cuh).  Host output goes through w.d_rec: [row_offsets | counts | pids] there, one
+// copy to page-locked staging, then to the caller's arrays.  *nnz > cap: ACG_E_OVERFLOW, nothing written.
+int count_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, int mode, uint64_t span_start,
+                  const uint64_t* d_offs, uint64_t n_docs, const BatchCounts& co, bool dev_out, uint64_t cap,
+                  uint64_t* nnz) {
+  Workspace& w = cur_ws();
+  const uint64_t n = t.n, nd1 = n_docs + 1;
+  const uint32_t pid_bits = uint32_t(acb::bit_width(std::max<uint64_t>(a->h.pattern_lens.size(), 1) - 1));
+  int rc;
+  float ms = 0;
+  // the time between ev2 and ev3, to order_ms
+  auto lap = [&]() -> int {
+    CK(cudaEventRecord(w.ev3, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+    w.stats.order_ms += ms;
+    return ACG_OK;
+  };
+  acb::CountRunsLaunch c{};
+  if (n) {
+    // tuples in buffer b: keys into the other one, sorted back into b; records: keys into 0, sorted into 1
+    const int b = t.keys ? sorted_buf : 1;
+    if (!t.keys && (rc = reserve_tuples(w, std::max<uint64_t>(n, w.tuple_cap())))) return rc;
+    if ((rc = reserve_all(std::max<uint64_t>(n, 1 << 16), w.d_scratch, w.d_flags))) return rc;
+    CK(cudaEventRecord(w.ev2, w.stream));
+    acb::CountKeysLaunch k;
+    k.t = t;
+    k.rec = t.keys ? nullptr : w.d_rec.p;
+    k.mode = mode;
+    k.span_start = span_start;
+    k.doc_offsets = d_offs;
+    k.n_docs = n_docs;
+    k.pid_bits = pid_bits;
+    k.keys_out = w.d_keys[1 - b];
+    k.pids_out = w.d_pids[1 - b];
+    CK(acb::launch_count_keys(k, w.stream));
+    const int end_bit = std::max(1, int(pid_bits) + acb::bit_width(n_docs - 1));
+    if ((rc = cub_call(w, [&](void* tmp, size_t& tb) {
+           return acb::sort_pairs(tmp, tb, w.d_keys[1 - b], w.d_keys[b], w.d_pids[1 - b], w.d_pids[b], n, end_bit,
+                                  w.stream);
+         })))
+      return rc;
+    c.keys = w.d_keys[b];
+    c.key_pids = w.d_pids[b];
+    c.n = n;
+    c.heads = reinterpret_cast<unsigned long long*>(w.d_keys[1 - b].p);  // the unsorted keys are spent
+    c.run_index = reinterpret_cast<unsigned long long*>(w.d_scratch.p);
+    c.pid_bits = pid_bits;
+    c.n_docs = n_docs;
+    CK(acb::launch_run_heads(c, w.stream));
+    if ((rc = cub_call(w, [&](void* tmp, size_t& tb) {
+           return acb::inclusive_sum_u64(tmp, tb, c.heads, c.run_index, n, w.stream);
+         })))
+      return rc;
+    CK(cudaMemcpyAsync(w.h_counter, c.run_index + n - 1, 8, cudaMemcpyDeviceToHost, w.stream));
+    if ((rc = lap())) return rc;
+    w.stats.launches += 11;  // keys, radix passes (upper bound), heads, scan
+    c.nnz = *w.h_counter;
+  }
+  *nnz = c.nnz;
+  if (c.nnz > cap) return ACG_E_OVERFLOW;
+  if (dev_out) {
+    c.row_offsets = co.row_offsets;
+    c.counts = co.counts;
+    c.pids = co.pids;
+  } else {
+    if ((rc = reserve_rec(w, std::max(nd1, c.nnz)))) return rc;  // 3 words each: room for 1 + 1 + 1/2 of them
+    c.row_offsets = w.d_rec;
+    c.counts = w.d_rec + nd1;
+    c.pids = reinterpret_cast<uint32_t*>(w.d_rec + nd1 + c.nnz);
+  }
+  CK(cudaEventRecord(w.ev2, w.stream));
+  if (n) {
+    CK(acb::launch_count_runs(c, w.stream));
+    CK(acb::launch_count_rows(c, w.stream));
+    w.stats.launches += 2;
+  } else {
+    CK(cudaMemsetAsync(c.row_offsets, 0, nd1 * 8, w.stream));
+  }
+  if ((rc = lap())) return rc;
+  if (dev_out) return ACG_OK;
+  const uint64_t bytes = nd1 * 8 + c.nnz * 12;
+  CK(cudaEventRecord(w.ev0, w.stream));
+  CK(cudaMemcpyAsync(w.h_rec, w.d_rec, bytes, cudaMemcpyDeviceToHost, w.stream));
+  CK(cudaEventRecord(w.ev1, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+  w.stats.d2h_ms += ms;
+  const uint8_t* h = reinterpret_cast<const uint8_t*>(w.h_rec.p);
+  CopyPool::get().copy(reinterpret_cast<uint8_t*>(co.row_offsets), h, nd1 * 8);
+  if (c.nnz) {
+    CopyPool::get().copy(reinterpret_cast<uint8_t*>(co.counts), h + nd1 * 8, c.nnz * 8);
+    CopyPool::get().copy(reinterpret_cast<uint8_t*>(co.pids), h + (nd1 + c.nnz) * 8, c.nnz * 4);
+  }
+  return ACG_OK;
+}
+
+// acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch / acg_find_batch (include/acb200.h), and
+// with `co` acg_pattern_counts_batch (what: kBatchFindIter or kBatchOverlapping, the records it counts; `cap` and
+// `n_out` are those of the counts).  is_match and find give one result per document: flags[n_docs] (find: found)
+// and, for find, out[n_docs].
 int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                const uint64_t* offs, uint64_t n_docs, int anchored, acg_match* out, uint64_t cap, uint64_t* n_out,
-               uint8_t* flags, int earliest = 0, const BatchDevOut* dv = nullptr) {
+               uint8_t* flags, int earliest = 0, const BatchDevOut* dv = nullptr, const BatchCounts* co = nullptr) {
   const bool per_doc = what == kBatchIsMatch || what == kBatchFind;
   if (!a || !offs || (per_doc ? n_docs && (!flags || (what == kBatchFind && !out)) : !n_out))
     return ACG_E_INVALID_ARG;
-  if (dv && !per_doc && (!dv->match_offsets || (!out && cap))) return ACG_E_INVALID_ARG;
+  if (co ? !co->row_offsets || ((!co->pids || !co->counts) && cap)
+         : dv && !per_doc && (!dv->match_offsets || (!out && cap)))
+    return ACG_E_INVALID_ARG;
   if (n_out) *n_out = 0;
   if (n_docs >= (1ull << 32)) return ACG_E_INVALID_ARG;
   const bool offs_on_device = dv && dv->offsets_on_device;
@@ -1441,7 +1552,10 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   }
   if ((rc = check_start(a->h, anchored))) return rc;
   if (!a->on_device) return ACG_E_NO_DEVICE;
-  if (n_docs == 0 && !dv) return ACG_OK;
+  if (n_docs == 0 && !dv) {
+    if (co) co->row_offsets[0] = 0;
+    return ACG_OK;
+  }
   earliest = find_earliest(a, anchored, earliest);
   const int engine = n_docs ? choose_engine(a, anchored, earliest, ACG_ENGINE_SEQUENTIAL, true) : ACG_ENGINE_SEQUENTIAL;
   if (engine < 0) return engine;
@@ -1459,17 +1573,19 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   unsigned long long* const d_incl = w.d_doc_incl;
   // The results go to the caller's device arrays, or to the workspace's and from there to the host at the end.
   // The records (find: one per document, at index doc) get their place once their number is known; on overflow
-  // nothing is written, and the caller retries with room for *n_out.
+  // nothing is written, and the caller retries with room for *n_out.  Records that are counted stay in the
+  // workspace.
   uint8_t* const d_flags = dv ? flags : w.d_doc_flags.p;
   uint64_t* const d_index = dv ? dv->match_offsets : reinterpret_cast<uint64_t*>(d_counts);
   uint64_t* d_rec = nullptr;
   uint64_t n_rec = 0;
   auto records = [&](uint64_t n) -> int {
-    if (n > cap) return ACG_E_OVERFLOW;
-    if (n && !out) return ACG_E_INVALID_ARG;
+    const bool to_caller = dv && !co;
+    if (!co && n > cap) return ACG_E_OVERFLOW;
+    if (!co && n && !out) return ACG_E_INVALID_ARG;
     n_rec = n;
-    const int e = dv ? ACG_OK : reserve_rec(w, n);
-    d_rec = dv ? reinterpret_cast<uint64_t*>(out) : w.d_rec.p;
+    const int e = to_caller ? ACG_OK : reserve_rec(w, n);
+    d_rec = to_caller ? reinterpret_cast<uint64_t*>(out) : w.d_rec.p;
     return e;
   };
   if (what == kBatchFind && (rc = records(n_docs))) return rc;
@@ -1490,7 +1606,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     CK(cudaMemcpyAsync(w.d_doc_offs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
   }
   if (n_docs == 0) {  // device output: the index of no records
-    if (!per_doc) CK(cudaMemsetAsync(dv->match_offsets, 0, 8, w.stream));
+    if (!per_doc) CK(cudaMemsetAsync(co ? co->row_offsets : dv->match_offsets, 0, 8, w.stream));
     CK(cudaStreamSynchronize(w.stream));
     return ACG_OK;
   }
@@ -1544,7 +1660,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     CK(cudaMemcpyAsync(w.h_counter, d_incl + n_docs - 1, 8, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaStreamSynchronize(w.stream));
     const uint64_t total = w.h_counter[0];
-    *n_out = total;
+    if (!co) *n_out = total;
     w.stats.raw_matches = total;
     w.stats.launches += 2;
     if ((rc = records(total))) return rc;
@@ -1556,6 +1672,12 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
       w.stats.launches += 1;
     }
     CK(cudaEventRecord(w.ev3, w.stream));
+    if (co) {
+      CK(cudaStreamSynchronize(w.stream));
+      cudaEventElapsedTime(&w.stats.scan_ms, w.ev2, w.ev3);
+      return count_matches(a, acb::TupleList{nullptr, nullptr, nullptr, total}, 0, 0, span_start, d_offs, n_docs, *co,
+                           dv != nullptr, cap, n_out);
+    }
     // the CSR index is the inclusive scan behind a zero
     CK(cudaMemsetAsync(d_index, 0, 8, w.stream));
     CK(cudaMemcpyAsync(d_index + 1, d_incl, n_docs * 8, cudaMemcpyDeviceToDevice, w.stream));
@@ -1567,7 +1689,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   DocBatch docs;
   docs.d_offsets = d_offs;
   docs.n = n_docs;
-  docs.unordered = per_doc;
+  docs.unordered = per_doc || (co && what == kBatchOverlapping);  // counts do not depend on the order
   TupleResult r;
   if ((rc = run_prefilter(a, pl.base, pl.readable, span_start, span_end, pf_mode, &r, pl.h_src, UINT64_MAX,
                           UINT64_MAX, &docs)))
@@ -1598,6 +1720,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     return finish(w.stats.order_ms);
   }
   if (what == kBatchFindIter && (rc = run_chain(a, chain_mode, &r))) return rc;
+  if (co)
+    return count_matches(a, tuple_list(a, w, r), r.sorted_buf, chain_mode, span_start, d_offs, n_docs, *co,
+                         dv != nullptr, cap, n_out);
   *n_out = r.n;
   if ((rc = records(r.n))) return rc;
   CK(cudaEventRecord(w.ev2, w.stream));
@@ -2010,6 +2135,24 @@ int acg_find_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len,
   dv.offsets_on_device = offsets_on_device != 0;
   return batch_impl(a, kBatchFind, static_cast<const uint8_t*>(d_hay), true, hay_len, doc_offsets, n_docs,
                     anchored, reinterpret_cast<acg_match*>(d_out), n_docs, nullptr, d_found, earliest != 0, &dv);
+}
+
+int acg_pattern_counts_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                             const uint64_t* doc_offsets, uint64_t n_docs, int anchored, int overlapping,
+                             uint64_t* row_offsets, uint32_t* pids, uint64_t* counts, uint64_t cap, uint64_t* nnz) {
+  const BatchCounts co{row_offsets, pids, counts};
+  return batch_impl(a, overlapping ? kBatchOverlapping : kBatchFindIter, hay, hay_on_device != 0, hay_len, doc_offsets,
+                    n_docs, anchored, nullptr, cap, nnz, nullptr, 0, nullptr, &co);
+}
+int acg_pattern_counts_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len, const uint64_t* doc_offsets,
+                                    int offsets_on_device, uint64_t n_docs, int anchored, int overlapping,
+                                    uint64_t* d_row_offsets, uint32_t* d_pids, uint64_t* d_counts, uint64_t cap,
+                                    uint64_t* nnz) {
+  BatchDevOut dv;
+  dv.offsets_on_device = offsets_on_device != 0;
+  const BatchCounts co{d_row_offsets, d_pids, d_counts};
+  return batch_impl(a, overlapping ? kBatchOverlapping : kBatchFindIter, static_cast<const uint8_t*>(d_hay), true,
+                    hay_len, doc_offsets, n_docs, anchored, nullptr, cap, nnz, nullptr, 0, &dv, &co);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

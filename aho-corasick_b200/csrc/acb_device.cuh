@@ -156,6 +156,42 @@ struct DocRecordsLaunch {
 };
 cudaError_t launch_doc_records(const DocRecordsLaunch& e, cudaStream_t s);
 
+// Pattern counts of a batch (acg_pattern_counts_batch): the n matches of a batch become a CSR matrix of
+// (document, pattern) counts in four steps -- a key doc << pid_bits | pid per match (launch_count_keys), a radix
+// sort of the keys (sort_pairs, end bit pid_bits + bits(n_docs - 1)), the runs of equal keys (launch_run_heads,
+// an inclusive scan of the heads, launch_count_runs) and the row index (launch_count_rows).
+struct CountKeysLaunch {
+  TupleList t;                  // prefilter engine: the tuples; t.n is the number of matches either way
+  const uint64_t* rec;          // sequential engine: [n * 3] acg_doc_match records (pid | doc << 32 first), else nullptr
+  int mode;                     // tuples: key layout as ChainLaunch::mode
+  uint64_t span_start;
+  const uint64_t* doc_offsets;  // tuples: [n_docs + 1]
+  uint64_t n_docs;
+  uint32_t pid_bits;            // bits of patterns_len - 1
+  uint64_t* keys_out;           // [n]
+  uint32_t* pids_out;           // [n]
+};
+cudaError_t launch_count_keys(const CountKeysLaunch& c, cudaStream_t s);
+// Over the n sorted keys: heads[i] = 1 where a run of equal keys starts; after run_index = inclusive scan of heads
+// (nnz = run_index[n - 1] runs), run r = run_index[i] - 1 of head i gets pids[r] and counts[r] (its length), and
+// row_offsets[d] (d <= n_docs) = the number of runs whose document is below d.  n > 0.
+struct CountRunsLaunch {
+  const uint64_t* keys;         // [n] ascending
+  const uint32_t* key_pids;     // [n] the pid of each key
+  uint64_t n;
+  unsigned long long* heads;    // [n]
+  unsigned long long* run_index;  // [n]
+  uint32_t pid_bits;
+  uint64_t n_docs;
+  uint64_t nnz;
+  uint32_t* pids;               // [nnz]
+  uint64_t* counts;             // [nnz]
+  uint64_t* row_offsets;        // [n_docs + 1]
+};
+cudaError_t launch_run_heads(const CountRunsLaunch& c, cudaStream_t s);
+cudaError_t launch_count_runs(const CountRunsLaunch& c, cudaStream_t s);
+cudaError_t launch_count_rows(const CountRunsLaunch& c, cudaStream_t s);
+
 // Offsets in device memory: result[0] = 1 if some offs[i] > offs[i + 1] or offs[n_docs] > hay_len (left as it
 // was otherwise: the caller clears it), result[1] = offs[0], result[2] = offs[n_docs].
 cudaError_t launch_check_offsets(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,

@@ -9,6 +9,10 @@
 //        doc_flags_kernel         per-document is_match / first match of a batch's
 //        doc_first_kernel         prefilter tuples
 //        doc_records_kernel       device-resident batch records + their CSR index by document
+//        count_keys_kernel        pattern counts of a batch: (document, pattern) keys, runs of
+//        run_heads_kernel         equal sorted keys, the CSR row index by document
+//        count_runs_kernel
+//        count_rows_kernel
 //        check_offsets_kernel     validation of document offsets in device memory
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
@@ -371,6 +375,60 @@ __global__ void doc_records_kernel(DocRecordsLaunch e) {
     for (d = doc + 1; d <= e.n_docs; ++d) e.match_offsets[d] = e.t.n;
 }
 
+// Pattern counts, step 1 (CountKeysLaunch): the (document, pattern) key of match i and its pid.
+__global__ void count_keys_kernel(CountKeysLaunch c) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.t.n) return;
+  uint64_t doc;
+  uint32_t pid;
+  if (c.rec) {
+    const uint64_t w0 = c.rec[i * 3];
+    pid = (uint32_t)w0;
+    doc = w0 >> 32;
+  } else {
+    pid = c.t.pids[i];
+    doc = doc_of(c.doc_offsets, c.n_docs, decode_key(c.t.keys[i], pid, c.mode, c.span_start, c.t.pattern_lens).start);
+  }
+  c.keys_out[i] = doc << c.pid_bits | pid;
+  c.pids_out[i] = pid;
+}
+
+// The first index in [lo, hi) whose key is >= v (hi if none); keys ascending.
+__device__ __forceinline__ uint64_t lower_bound_key(const uint64_t* keys, uint64_t lo, uint64_t hi, uint64_t v) {
+  while (lo < hi) {
+    const uint64_t mid = lo + ((hi - lo) >> 1);
+    if (keys[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void run_heads_kernel(CountRunsLaunch c) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.n) return;
+  c.heads[i] = i == 0 || c.keys[i] != c.keys[i - 1];
+}
+
+// The head of each run writes its entry: the pid, and the run's length -- the next head's start (the first
+// greater key, or n after the last run) minus its own.
+__global__ void count_runs_kernel(CountRunsLaunch c) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.n) return;
+  const uint64_t key = c.keys[i];
+  if (i && c.keys[i - 1] == key) return;
+  const uint64_t r = c.run_index[i] - 1;
+  c.pids[r] = c.key_pids[i];
+  c.counts[r] = lower_bound_key(c.keys, i + 1, c.n, key + 1) - i;
+}
+
+// One thread per document d <= n_docs: the first key of a document >= d heads a run, whose index is the number
+// of runs before it (nnz when there is none).
+__global__ void count_rows_kernel(CountRunsLaunch c) {
+  const uint64_t d = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (d > c.n_docs) return;
+  const uint64_t i = lower_bound_key(c.keys, 0, c.n, d << c.pid_bits);
+  c.row_offsets[d] = i < c.n ? c.run_index[i] - 1 : c.nnz;
+}
+
 __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
                                      unsigned long long* result) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -482,6 +540,27 @@ cudaError_t launch_doc_first(const DocFlagsLaunch& f, cudaStream_t s) {
 cudaError_t launch_doc_records(const DocRecordsLaunch& e, cudaStream_t s) {
   if (e.t.n == 0) return cudaSuccess;
   ACB_LAUNCH(doc_records_kernel, (unsigned)((e.t.n + 255) / 256), 256, 0, s, e);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_count_keys(const CountKeysLaunch& c, cudaStream_t s) {
+  if (c.t.n == 0) return cudaSuccess;
+  ACB_LAUNCH(count_keys_kernel, (unsigned)((c.t.n + 255) / 256), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_run_heads(const CountRunsLaunch& c, cudaStream_t s) {
+  ACB_LAUNCH(run_heads_kernel, (unsigned)((c.n + 255) / 256), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_count_runs(const CountRunsLaunch& c, cudaStream_t s) {
+  ACB_LAUNCH(count_runs_kernel, (unsigned)((c.n + 255) / 256), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_count_rows(const CountRunsLaunch& c, cudaStream_t s) {
+  ACB_LAUNCH(count_rows_kernel, (unsigned)((c.n_docs + 1 + 255) / 256), 256, 0, s, c);
   return cudaGetLastError();
 }
 

@@ -262,6 +262,28 @@ int acg_find_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_le
                           const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
                           int anchored, int earliest, acg_doc_match* d_out, uint8_t* d_found);
 
+/* How often each pattern occurs in each document of a batch, as a sparse CSR matrix
+ * [n_docs x patterns_len].  Let R be the records acg_find_overlapping_batch (overlapping != 0) or
+ * acg_find_iter_batch (overlapping == 0) returns for the same dfa, haystack, offsets and anchored.
+ * Document d's entries are pids[row_offsets[d] .. row_offsets[d + 1]), strictly ascending;
+ * counts[i] (>= 1) is the number of records of R with doc == d and pid == pids[i].
+ * *nnz = row_offsets[n_docs] = number of distinct (doc, pid) pairs in R.
+ * row_offsets has n_docs + 1 entries, pids and counts cap entries each.  If *nnz > cap the call
+ * returns ACG_E_OVERFLOW with the required count in *nnz and writes none of the three arrays;
+ * cap == 0 with NULL pids / counts is a size query.  Error codes, their order and the engine are
+ * those of the batch call `overlapping` selects.  The counts are computed on the device without
+ * materialising the records: the result's size depends on the number of distinct pairs only.
+ * _devout: the three arrays are device pointers, doc_offsets as in the other _devout calls; nnz is
+ * a host pointer. */
+int acg_pattern_counts_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                             const uint64_t* doc_offsets, uint64_t n_docs, int anchored, int overlapping,
+                             uint64_t* row_offsets, uint32_t* pids, uint64_t* counts, uint64_t cap,
+                             uint64_t* nnz);
+int acg_pattern_counts_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_len,
+                                    const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                                    int anchored, int overlapping, uint64_t* d_row_offsets,
+                                    uint32_t* d_pids, uint64_t* d_counts, uint64_t cap, uint64_t* nnz);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

@@ -351,6 +351,37 @@ class AhoCorasick {
                          bool earliest = false) const {
     return std::move(try_find_batch(haystack, offsets, a, earliest).unwrap());
   }
+  // How often each pattern occurs in each document (acg_pattern_counts_batch): the records of
+  // find_overlapping_iter_batch (`overlapping`) or find_iter_batch counted by (document, pattern), as a CSR
+  // matrix -- document d's patterns are pids[row_offsets[d] .. row_offsets[d + 1]), ascending, each counts[i] times.
+  struct PatternCounts {
+    std::vector<uint64_t> row_offsets;  // [n_docs + 1]
+    std::vector<uint32_t> pids;
+    std::vector<uint64_t> counts;
+  };
+  Result<PatternCounts> try_pattern_counts_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                                 bool overlapping = false, Anchored a = Anchored::No) const {
+    Result<PatternCounts> r;
+    if (offsets.empty()) { r.error = ACG_E_INVALID_ARG; return r; }
+    PatternCounts& c = r.value;
+    c.row_offsets.resize(offsets.size());
+    uint64_t nnz = 0;
+    for (uint64_t cap = cap_hint_;; cap = nnz) {
+      c.pids.resize(cap);
+      c.counts.resize(cap);
+      r.error = acg_pattern_counts_batch(h_, reinterpret_cast<const uint8_t*>(haystack.data()), 0, haystack.size(),
+                                         offsets.data(), offsets.size() - 1, int(a), int(overlapping),
+                                         c.row_offsets.data(), c.pids.data(), c.counts.data(), cap, &nnz);
+      if (r.error != ACG_E_OVERFLOW) break;  // two-call protocol: nnz is the required count
+    }
+    c.pids.resize(r.error ? 0 : nnz);
+    c.counts.resize(r.error ? 0 : nnz);
+    return r;
+  }
+  PatternCounts pattern_counts_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                     bool overlapping = false, Anchored a = Anchored::No) const {
+    return std::move(try_pattern_counts_batch(haystack, offsets, overlapping, a).unwrap());
+  }
 
   // replace_all_with / replace_all_with_bytes, :834 / :887 (src/automaton.rs:498-550)
   template <class F>

@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
-"""Batched search over many documents in one device call (acg_find_overlapping_batch, acg_find_batch).
+"""Batched search over many documents in one device call (acg_find_overlapping_batch, acg_find_batch,
+acg_pattern_counts_batch).
 
     python tools/bench_docs.py [--hay-gib 4] [--steps 20] [--warmup 5] [--engine 0]
-                               [--call overlapping|find] [--workload cfg2|cfg3] [--out host|device]
+                               [--call overlapping|find|counts] [--workload cfg2|cfg3] [--out host|device]
 
 cfg 2's automaton and haystack (same seeds as bench.py), device-resident, cut at seeded boundaries into
 documents of log-uniform length in [16 B, 16 KiB] (~1.8 M documents, mean ~2.4 KiB at 4 GiB).  Prints one
@@ -22,6 +23,13 @@ calls against one find_batch call over the same documents (host haystack, same r
 find_batch_torch, acg_*_batch_devout): offsets a CUDA tensor, results left in device memory.  Its results are
 checked equal to the host-output call's, and the checks above then run as usual.  wall_ms_per_step (host
 clock around calls that end in a device synchronise) is the number to compare between --out host and device.
+
+--call counts times pattern_counts_batch (how often each pattern occurs in each document: cfg 2 counts
+find_overlapping_iter, cfg 3 find_iter) against what a caller does without it, in the same session on the same
+documents: the device records (find_overlapping_iter_batch_torch / find_iter_batch_torch) grouped with
+torch.unique(doc * P + pid, return_counts=True).  Both give the same matrix (checked).  Device time is measured
+with CUDA events around each whole sequence; the counts call's own scan_ms + order_ms are reported too.
+--out host: the counts go to host memory (pattern_counts_batch_np); device: a CUDA sparse CSR tensor.
 """
 import argparse
 import importlib.util
@@ -129,13 +137,80 @@ def bench_find(args, ac, d_hay, offs, ClockSampler):
         "clocks": clocks.summary()}), flush=True)
 
 
+def bench_counts(args, ac, d_hay, offs, ClockSampler):
+    """--call counts: pattern_counts_batch, and the records + torch.unique path, alternated step by step."""
+    import numpy as np
+    import torch
+    n, n_docs, n_pats = d_hay.numel(), offs.size - 1, ac.patterns_len()
+    overlapping = args.workload == "cfg2"
+    d_offs = torch.from_numpy(offs).cuda()
+    if args.out == "device":
+        counts_call = lambda: ac.pattern_counts_batch_torch((d_hay, d_offs), overlapping=overlapping)  # noqa: E731
+    else:
+        counts_call = lambda: ac.pattern_counts_batch_np((d_hay, offs), overlapping=overlapping)  # noqa: E731
+    records = ac.find_overlapping_iter_batch_torch if overlapping else ac.find_iter_batch_torch
+
+    def records_call():
+        r = records((d_hay, d_offs))
+        return torch.unique(r.doc * n_pats + r.pid, return_counts=True)
+
+    def timed(call):
+        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0 = time.perf_counter()
+        start.record()
+        out = call()
+        end.record()
+        end.synchronize()
+        return out, start.elapsed_time(end), (time.perf_counter() - t0) * 1e3
+
+    for _ in range(args.warmup):
+        counts_call()
+        records_call()
+    c_dev, c_wall, c_lib, r_dev, r_wall = [], [], [], [], []
+    with ClockSampler(0) as clocks:
+        for _ in range(args.steps):
+            got, dev_ms, wall_ms = timed(counts_call)
+            st = ac.last_stats()
+            c_dev.append(dev_ms)
+            c_wall.append(wall_ms)
+            c_lib.append(st["scan_ms"] + st["order_ms"])
+            (keys, cnt), dev_ms, wall_ms = timed(records_call)
+            r_dev.append(dev_ms)
+            r_wall.append(wall_ms)
+    engine = int(st["engine"])
+    # the same matrix: CSR entries as doc * P + pid keys, in the same (ascending) order
+    if args.out == "device":
+        rows, pids, counts = got.crow_indices(), got.col_indices(), got.values()
+    else:
+        rows, pids, counts = (torch.from_numpy(a.astype(np.int64)).cuda() for a in got)
+    doc = torch.repeat_interleave(torch.arange(n_docs, device="cuda"), rows[1:] - rows[:-1])
+    assert torch.equal(doc * n_pats + pids, keys) and torch.equal(counts, cnt), "counts differ from torch.unique"
+    med = lambda v: float(np.median(v))  # noqa: E731
+    what = "find_overlapping_iter" if overlapping else "find_iter"
+    print(json.dumps({
+        "metric": "pattern_counts_device_ms", "value": med(c_dev), "unit": "ms",
+        "steps": args.steps, "warmup": args.warmup,
+        "workload": f"{args.workload}'s automaton and haystack cut into documents of log-uniform length in "
+                    f"[16 B, 16 KiB], {what} of every document counted by (document, pattern)",
+        "haystack_bytes": n, "documents": n_docs, "patterns": n_pats, "out": args.out,
+        "engine": {2: "prefilter", 3: "sequential"}.get(engine, engine),
+        "nnz": int(rows[-1]), "matches": int(st["raw_matches"]),
+        "counts_call": {"device_ms": med(c_dev), "wall_ms": med(c_wall), "scan_plus_order_ms": med(c_lib),
+                        "scan_ms": float(st["scan_ms"]), "order_ms": float(st["order_ms"])},
+        "records_then_torch_unique": {"device_ms": med(r_dev), "wall_ms": med(r_wall)},
+        "timing": "medians; device_ms: CUDA events around each whole sequence; wall_ms: host clock around calls "
+                  "that end in a device synchronise; scan_plus_order_ms: the counts call's own CUDA events",
+        "check": {"equal_to_torch_unique": True},
+        "clocks": clocks.summary()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--hay-gib", type=float, default=4.0)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--engine", type=int, default=0, help="0 auto, 3 the per-document sequential kernel")
-    ap.add_argument("--call", default="overlapping", choices=["overlapping", "find"])
+    ap.add_argument("--call", default="overlapping", choices=["overlapping", "find", "counts"])
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg3"])
     ap.add_argument("--out", default="host", choices=["host", "device"],
                     help="results to host memory (acg_*_batch) or left in device memory (acg_*_batch_devout)")
@@ -161,6 +236,8 @@ def main():
     offs = W.doc_offsets(n, 0xD0C5)
     if args.call == "find":
         return bench_find(args, ac, d_hay, offs, ClockSampler)
+    if args.call == "counts":
+        return bench_counts(args, ac, d_hay, offs, ClockSampler)
     batch = (d_hay, offs)
     call = ac.find_overlapping_iter_batch_np
     if args.out == "device":
