@@ -163,6 +163,8 @@ def _declare(lib):
                                              C.POINTER(_u64)]
     lib.acg_pattern_counts_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _i, _vp, _vp, _vp, _u64,
                                                     C.POINTER(_u64)]
+    lib.acg_match_coverage_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _i, _vp, _vp]
+    lib.acg_match_coverage_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _i, _vp, _vp]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -930,6 +932,49 @@ class AhoCorasick:
                 self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs, int(anchored), int(overlapping),
                 rows.data_ptr(), pids.data_ptr(), counts.data_ptr(), cap, nnz))
         return torch.sparse_csr_tensor(rows, pids.to(torch.int64), counts, size=(n_docs, self.patterns_len()))
+
+    # ---- match coverage per document (acg_match_coverage_batch) ----
+    # How much of each document the records of find_overlapping_iter_batch (overlapping) or find_iter_batch cover:
+    # the bytes inside at least one match, per document, and optionally the per-byte mask, from the device.
+    def match_coverage_batch_np(self, docs, overlapping=False, anchored=Anchored.No, mask=False):
+        """covered, uint64 [n_docs]: the bytes of each document inside at least one of its matches (empty matches
+        cover nothing).  With mask=True also a bool array the length of the values buffer, True where a byte lies
+        in a match of its document (False outside [offsets[0], offsets[-1])).  `docs` as in find_iter_batch_np."""
+        keep, ptr, n, on_dev, offs = _batch_input(docs)
+        n_docs = offs.size - 1
+        covered = np.empty(n_docs, dtype=np.uint64)
+        m = np.zeros(n, dtype=np.uint8) if mask else None
+        rc = _lib.acg_match_coverage_batch(self._h, ptr, on_dev, n, offs.ctypes.data, n_docs, int(anchored),
+                                           int(overlapping), covered.ctypes.data, m.ctypes.data if mask else None)
+        if rc:
+            self._raise(rc)
+        return (covered, m.view(bool)) if mask else covered
+
+    def match_coverage_batch_devout(self, d_hay_ptr, hay_len, offsets, covered_ptr, mask_ptr=None, overlapping=False,
+                                    anchored=Anchored.No, n_docs=None):
+        """The coverage into device memory: covered_ptr [n_docs] uint64 and, unless mask_ptr is None, the mask
+        (uint8, indexed like the haystack: only [offsets[0], offsets[n_docs]) is written)."""
+        keep, optr, n_docs, on_dev = _devout_offsets(offsets, n_docs)
+        rc = _lib.acg_match_coverage_batch_devout(self._h, d_hay_ptr, hay_len, optr, on_dev, n_docs, int(anchored),
+                                                  int(overlapping), covered_ptr, mask_ptr)
+        if rc:
+            self._raise(rc)
+
+    def match_coverage_batch_torch(self, docs, overlapping=False, anchored=Anchored.No, mask=True):
+        """(covered, CUDA int64 [n_docs]; mask, CUDA bool [values.numel()] or None) on the values' device.  The
+        mask is False outside [offsets[0], offsets[-1]).  `docs` as in find_iter_batch_torch."""
+        import torch
+        values, keep, optr, n_docs, on_dev = _torch_batch(docs)
+        covered = torch.empty(n_docs, dtype=torch.int64, device=values.device)
+        m = torch.zeros(values.numel(), dtype=torch.bool, device=values.device) if mask else None
+        if mask:
+            torch.cuda.current_stream(values.device).synchronize()  # the zeros are written before the call's own
+        rc = _lib.acg_match_coverage_batch_devout(self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs,
+                                                  int(anchored), int(overlapping), covered.data_ptr(),
+                                                  m.data_ptr() if mask else None)
+        if rc:
+            self._raise(rc)
+        return covered, m
 
     # ---- replace / stream: host-side glue over find_iter, as in the reference -------------------
     @staticmethod

@@ -1521,18 +1521,140 @@ int count_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, int
   return ACG_OK;
 }
 
+// acg_match_coverage_batch(_devout): instead of the records of a find_iter / overlapping batch, the bytes of each
+// document they cover (host or device arrays, as the call's other outputs).
+struct BatchCoverage {
+  uint64_t* covered;  // [n_docs]
+  uint8_t* mask;      // indexed like the haystack, or nullptr
+};
+
+// The mask of [lo, hi), written on the device at d_mask + lo, copied to the host array h_mask + lo: in one copy
+// when that is page-locked, else chunk by chunk through the workspace's staging ring (two page-locked buffers of
+// one pipeline chunk), each chunk's copy to the caller overlapping the next one's transfer.
+int copy_mask_out(const acg_dfa* a, const uint8_t* d_mask, uint8_t* h_mask, uint64_t lo, uint64_t hi) {
+  Workspace& w = cur_ws();
+  if (!is_pageable_host(h_mask + lo)) {
+    CK(cudaMemcpyAsync(h_mask + lo, d_mask + lo, hi - lo, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    return ACG_OK;
+  }
+  const uint64_t chunk = std::min<uint64_t>(a->pipeline_chunk, hi - lo);
+  int rc = reserve_stage(w, chunk);
+  if (rc) return rc;
+  uint64_t at[2] = {0, 0}, len[2] = {0, 0};
+  auto drain = [&](int i) -> int {
+    if (!len[i]) return ACG_OK;
+    CK(cudaEventSynchronize(w.stage_ev[i]));
+    CopyPool::get().copy(h_mask + at[i], w.h_stage[i], size_t(len[i]));
+    len[i] = 0;
+    return ACG_OK;
+  };
+  int i = 0;
+  for (uint64_t c0 = lo; c0 < hi; c0 += chunk, i ^= 1) {
+    if ((rc = drain(i))) return rc;
+    at[i] = c0;
+    len[i] = std::min(chunk, hi - c0);
+    CK(cudaMemcpyAsync(w.h_stage[i], d_mask + c0, len[i], cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaEventRecord(w.stage_ev[i], w.stream));
+  }
+  if ((rc = drain(i))) return rc;  // the older chunk first
+  return drain(i ^ 1);
+}
+
+// The n matches of a batch -- the tuples `t` of the prefilter engine, or (t.keys == nullptr) the records the
+// sequential engine left at w.d_rec -- turned into the bytes of each document they cover, and the mask (CoverLaunch,
+// acb_device.cuh).  `ordered`: the matches are in start order already (find_iter), so there is no sort.  Scratch:
+// (start, length) pairs in the tuple buffers, ends in w.d_scratch.  Host output: the counts in w.d_doc_counts and
+// the mask in the haystack staging buffer (the haystack is spent by now), copied to the caller from there.
+int cover_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, int mode, bool ordered,
+                  uint64_t span_start, uint64_t span_end, const uint64_t* d_offs, uint64_t n_docs,
+                  const BatchCoverage& cv, bool dev_out) {
+  Workspace& w = cur_ws();
+  const uint64_t n = t.n;
+  int rc;
+  acb::CoverLaunch c{};
+  c.t = t;
+  c.rec = t.keys ? nullptr : w.d_rec.p;
+  c.mode = mode;
+  c.span_start = span_start;
+  c.doc_offsets = d_offs;
+  c.n_docs = n_docs;
+  c.covered = dev_out ? reinterpret_cast<unsigned long long*>(cv.covered) : w.d_doc_counts.p;
+  c.mask = cv.mask;
+  if (cv.mask && !dev_out) {
+    const uint8_t* base = nullptr;
+    if ((rc = stage_host_span(a, nullptr, span_start, span_end, &base, true))) return rc;
+    c.mask = const_cast<uint8_t*>(base);
+  }
+  // tuples in buffer b: (start, length) into the other one, sorted back into b; records: into 0, sorted into 1
+  const int b = t.keys ? sorted_buf : 1;
+  if (n) {
+    if (!t.keys && (rc = reserve_tuples(w, std::max<uint64_t>(n, w.tuple_cap())))) return rc;
+    if ((rc = reserve_all(std::max<uint64_t>(n, 1 << 16), w.d_scratch, w.d_flags))) return rc;
+  }
+  CK(cudaEventRecord(w.ev2, w.stream));
+  CK(cudaMemsetAsync(c.covered, 0, n_docs * 8, w.stream));
+  if (c.mask) CK(cudaMemsetAsync(c.mask + span_start, 0, span_end - span_start, w.stream));
+  if (n) {
+    c.starts = w.d_keys[1 - b];
+    c.lens = w.d_pids[1 - b];
+    c.max_end = w.d_scratch;
+    CK(acb::launch_cover_keys(c, w.stream));
+    w.stats.launches += 1;
+    if (!ordered) {
+      const int end_bit = std::max(1, acb::bit_width(span_end - span_start));
+      if ((rc = cub_call(w, [&](void* tmp, size_t& tb) {
+             return acb::sort_pairs(tmp, tb, w.d_keys[1 - b], w.d_keys[b], w.d_pids[1 - b], w.d_pids[b], n, end_bit,
+                                    w.stream);
+           })))
+        return rc;
+      c.starts = w.d_keys[b];
+      c.lens = w.d_pids[b];
+      w.stats.launches += 8;  // radix passes (upper bound)
+    }
+    CK(acb::launch_cover_ends(c, w.stream));
+    if ((rc = cub_call(w, [&](void* tmp, size_t& tb) { return acb::scan_max_u64(tmp, tb, c.max_end, n, w.stream); })))
+      return rc;
+    CK(acb::launch_cover_runs(c, w.stream));
+    w.stats.launches += 3;  // ends, scan, runs
+    if (c.mask) {
+      CK(acb::launch_cover_mask(c, w.stream));
+      w.stats.launches += 1;
+    }
+  }
+  CK(cudaEventRecord(w.ev3, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+  w.stats.order_ms += ms;
+  if (dev_out) return ACG_OK;
+  if ((rc = reserve_rec(w, (n_docs + 2) / 3))) return rc;  // 3 words per record: room for n_docs words
+  CK(cudaEventRecord(w.ev0, w.stream));
+  CK(cudaMemcpyAsync(w.h_rec, c.covered, n_docs * 8, cudaMemcpyDeviceToHost, w.stream));
+  if (cv.mask && (rc = copy_mask_out(a, c.mask, cv.mask, span_start, span_end))) return rc;
+  CK(cudaEventRecord(w.ev1, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+  w.stats.d2h_ms += ms;
+  CopyPool::get().copy(reinterpret_cast<uint8_t*>(cv.covered), reinterpret_cast<const uint8_t*>(w.h_rec.p),
+                       n_docs * 8);
+  return ACG_OK;
+}
+
 // acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch / acg_find_batch (include/acb200.h), and
-// with `co` acg_pattern_counts_batch (what: kBatchFindIter or kBatchOverlapping, the records it counts; `cap` and
-// `n_out` are those of the counts).  is_match and find give one result per document: flags[n_docs] (find: found)
-// and, for find, out[n_docs].
+// with `co` acg_pattern_counts_batch or with `cv` acg_match_coverage_batch (what: kBatchFindIter or
+// kBatchOverlapping, the records they aggregate; `cap` and `n_out` are those of the counts).  is_match and find
+// give one result per document: flags[n_docs] (find: found) and, for find, out[n_docs].
 int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                const uint64_t* offs, uint64_t n_docs, int anchored, acg_match* out, uint64_t cap, uint64_t* n_out,
-               uint8_t* flags, int earliest = 0, const BatchDevOut* dv = nullptr, const BatchCounts* co = nullptr) {
+               uint8_t* flags, int earliest = 0, const BatchDevOut* dv = nullptr, const BatchCounts* co = nullptr,
+               const BatchCoverage* cv = nullptr) {
   const bool per_doc = what == kBatchIsMatch || what == kBatchFind;
   if (!a || !offs || (per_doc ? n_docs && (!flags || (what == kBatchFind && !out)) : !n_out))
     return ACG_E_INVALID_ARG;
-  if (co ? !co->row_offsets || ((!co->pids || !co->counts) && cap)
-         : dv && !per_doc && (!dv->match_offsets || (!out && cap)))
+  if (cv ? n_docs && !cv->covered
+         : co ? !co->row_offsets || ((!co->pids || !co->counts) && cap)
+              : dv && !per_doc && (!dv->match_offsets || (!out && cap)))
     return ACG_E_INVALID_ARG;
   if (n_out) *n_out = 0;
   if (n_docs >= (1ull << 32)) return ACG_E_INVALID_ARG;
@@ -1573,16 +1695,17 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   unsigned long long* const d_incl = w.d_doc_incl;
   // The results go to the caller's device arrays, or to the workspace's and from there to the host at the end.
   // The records (find: one per document, at index doc) get their place once their number is known; on overflow
-  // nothing is written, and the caller retries with room for *n_out.  Records that are counted stay in the
-  // workspace.
+  // nothing is written, and the caller retries with room for *n_out.  Records that are counted or covered stay
+  // in the workspace.
   uint8_t* const d_flags = dv ? flags : w.d_doc_flags.p;
   uint64_t* const d_index = dv ? dv->match_offsets : reinterpret_cast<uint64_t*>(d_counts);
   uint64_t* d_rec = nullptr;
   uint64_t n_rec = 0;
+  const bool aggregated = co || cv;
   auto records = [&](uint64_t n) -> int {
-    const bool to_caller = dv && !co;
-    if (!co && n > cap) return ACG_E_OVERFLOW;
-    if (!co && n && !out) return ACG_E_INVALID_ARG;
+    const bool to_caller = dv && !aggregated;
+    if (!aggregated && n > cap) return ACG_E_OVERFLOW;
+    if (!aggregated && n && !out) return ACG_E_INVALID_ARG;
     n_rec = n;
     const int e = to_caller ? ACG_OK : reserve_rec(w, n);
     d_rec = to_caller ? reinterpret_cast<uint64_t*>(out) : w.d_rec.p;
@@ -1606,7 +1729,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     CK(cudaMemcpyAsync(w.d_doc_offs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
   }
   if (n_docs == 0) {  // device output: the index of no records
-    if (!per_doc) CK(cudaMemsetAsync(co ? co->row_offsets : dv->match_offsets, 0, 8, w.stream));
+    if (!per_doc && !cv) CK(cudaMemsetAsync(co ? co->row_offsets : dv->match_offsets, 0, 8, w.stream));
     CK(cudaStreamSynchronize(w.stream));
     return ACG_OK;
   }
@@ -1672,11 +1795,14 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
       w.stats.launches += 1;
     }
     CK(cudaEventRecord(w.ev3, w.stream));
-    if (co) {
+    if (aggregated) {
       CK(cudaStreamSynchronize(w.stream));
       cudaEventElapsedTime(&w.stats.scan_ms, w.ev2, w.ev3);
-      return count_matches(a, acb::TupleList{nullptr, nullptr, nullptr, total}, 0, 0, span_start, d_offs, n_docs, *co,
-                           dv != nullptr, cap, n_out);
+      const acb::TupleList recs{nullptr, nullptr, nullptr, total};
+      if (cv)  // find_iter records are in start order; overlapping ones in end order
+        return cover_matches(a, recs, 0, 0, what == kBatchFindIter, span_start, span_end, d_offs, n_docs, *cv,
+                             dv != nullptr);
+      return count_matches(a, recs, 0, 0, span_start, d_offs, n_docs, *co, dv != nullptr, cap, n_out);
     }
     // the CSR index is the inclusive scan behind a zero
     CK(cudaMemsetAsync(d_index, 0, 8, w.stream));
@@ -1689,7 +1815,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   DocBatch docs;
   docs.d_offsets = d_offs;
   docs.n = n_docs;
-  docs.unordered = per_doc || (co && what == kBatchOverlapping);  // counts do not depend on the order
+  docs.unordered = per_doc || (aggregated && what == kBatchOverlapping);  // counts and coverage do not depend on it
   TupleResult r;
   if ((rc = run_prefilter(a, pl.base, pl.readable, span_start, span_end, pf_mode, &r, pl.h_src, UINT64_MAX,
                           UINT64_MAX, &docs)))
@@ -1720,6 +1846,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     return finish(w.stats.order_ms);
   }
   if (what == kBatchFindIter && (rc = run_chain(a, chain_mode, &r))) return rc;
+  if (cv)  // the tuples of find_iter are in start order: the chain's matches neither overlap nor go backwards
+    return cover_matches(a, tuple_list(a, w, r), r.sorted_buf, chain_mode, what == kBatchFindIter, span_start,
+                         span_end, d_offs, n_docs, *cv, dv != nullptr);
   if (co)
     return count_matches(a, tuple_list(a, w, r), r.sorted_buf, chain_mode, span_start, d_offs, n_docs, *co,
                          dv != nullptr, cap, n_out);
@@ -2153,6 +2282,25 @@ int acg_pattern_counts_batch_devout(const acg_dfa* a, const void* d_hay, uint64_
   const BatchCounts co{d_row_offsets, d_pids, d_counts};
   return batch_impl(a, overlapping ? kBatchOverlapping : kBatchFindIter, static_cast<const uint8_t*>(d_hay), true,
                     hay_len, doc_offsets, n_docs, anchored, nullptr, cap, nnz, nullptr, 0, &dv, &co);
+}
+
+int acg_match_coverage_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                             const uint64_t* doc_offsets, uint64_t n_docs, int anchored, int overlapping,
+                             uint64_t* covered, uint8_t* mask) {
+  const BatchCoverage cv{covered, mask};
+  uint64_t unused = 0;
+  return batch_impl(a, overlapping ? kBatchOverlapping : kBatchFindIter, hay, hay_on_device != 0, hay_len, doc_offsets,
+                    n_docs, anchored, nullptr, 0, &unused, nullptr, 0, nullptr, nullptr, &cv);
+}
+int acg_match_coverage_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len, const uint64_t* doc_offsets,
+                                    int offsets_on_device, uint64_t n_docs, int anchored, int overlapping,
+                                    uint64_t* d_covered, uint8_t* d_mask) {
+  BatchDevOut dv;
+  dv.offsets_on_device = offsets_on_device != 0;
+  const BatchCoverage cv{d_covered, d_mask};
+  uint64_t unused = 0;
+  return batch_impl(a, overlapping ? kBatchOverlapping : kBatchFindIter, static_cast<const uint8_t*>(d_hay), true,
+                    hay_len, doc_offsets, n_docs, anchored, nullptr, 0, &unused, nullptr, 0, &dv, nullptr, &cv);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

@@ -192,6 +192,32 @@ cudaError_t launch_run_heads(const CountRunsLaunch& c, cudaStream_t s);
 cudaError_t launch_count_runs(const CountRunsLaunch& c, cudaStream_t s);
 cudaError_t launch_count_rows(const CountRunsLaunch& c, cudaStream_t s);
 
+// Match coverage of a batch (acg_match_coverage_batch): the n matches of a batch become, per document, the number
+// of bytes inside at least one match, and optionally a byte mask of those bytes.  Steps: (start - span_start,
+// length) per match (launch_cover_keys); a radix sort by start unless the matches are in start order already
+// (sort_pairs); the ends and their running maximum M (launch_cover_ends, scan_max_u64 in place); match i adds
+// e_i - max(s_i, M_{i-1}) when positive (M_{-1} = 0) to the count of its document (launch_cover_runs), and writes
+// those bytes of the mask (launch_cover_mask).  The parts [max(s_i, M_{i-1}), e_i) are disjoint and their union is
+// the union of the matches; no match crosses a document end, so no running maximum carries a document's end
+// past a later document's starts.
+struct CoverLaunch {
+  TupleList t;                  // prefilter engine: the tuples; t.n is the number of matches either way
+  const uint64_t* rec;          // sequential engine: [n * 3] acg_doc_match records, else nullptr
+  int mode;                     // tuples: key layout as ChainLaunch::mode
+  uint64_t span_start;
+  const uint64_t* doc_offsets;  // [n_docs + 1]
+  uint64_t n_docs;
+  uint64_t* starts;             // [n] start - span_start
+  uint32_t* lens;               // [n]
+  uint64_t* max_end;            // [n] end - span_start, then its inclusive running maximum
+  unsigned long long* covered;  // [n_docs], zeroed by the caller
+  uint8_t* mask;                // indexed with haystack offsets, [span_start, span_end) zeroed; nullptr: none
+};
+cudaError_t launch_cover_keys(const CoverLaunch& c, cudaStream_t s);
+cudaError_t launch_cover_ends(const CoverLaunch& c, cudaStream_t s);
+cudaError_t launch_cover_runs(const CoverLaunch& c, cudaStream_t s);
+cudaError_t launch_cover_mask(const CoverLaunch& c, cudaStream_t s);
+
 // Offsets in device memory: result[0] = 1 if some offs[i] > offs[i + 1] or offs[n_docs] > hay_len (left as it
 // was otherwise: the caller clears it), result[1] = offs[0], result[2] = offs[n_docs].
 cudaError_t launch_check_offsets(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,

@@ -13,6 +13,10 @@
 //        run_heads_kernel         equal sorted keys, the CSR row index by document
 //        count_runs_kernel
 //        count_rows_kernel
+//        cover_keys_kernel        match coverage of a batch: (start, length) per match, ends,
+//        cover_ends_kernel        each match's uncovered part counted per document and written
+//        cover_runs_kernel        to the byte mask
+//        cover_mask_kernel
 //        check_offsets_kernel     validation of document offsets in device memory
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
@@ -429,6 +433,70 @@ __global__ void count_rows_kernel(CountRunsLaunch c) {
   c.row_offsets[d] = i < c.n ? c.run_index[i] - 1 : c.nnz;
 }
 
+// Match coverage, step 1 (CoverLaunch): the start of match i relative to the span, and its length.
+__global__ void cover_keys_kernel(CoverLaunch c) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.t.n) return;
+  uint64_t start, len;
+  if (c.rec) {
+    const uint64_t* r = c.rec + i * 3;
+    start = c.doc_offsets[r[0] >> 32] - c.span_start + r[1];
+    len = r[2] - r[1];
+  } else {
+    const MatchSpan m = decode_key(c.t.keys[i], c.t.pids[i], c.mode, c.span_start, c.t.pattern_lens);
+    start = m.start - c.span_start;
+    len = m.end - m.start;
+  }
+  c.starts[i] = start;
+  c.lens[i] = (uint32_t)len;
+}
+
+__global__ void cover_ends_kernel(CoverLaunch c) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.t.n) return;
+  c.max_end[i] = c.starts[i] + c.lens[i];
+}
+
+// The part of match i that no earlier match covers: [max(s_i, M_{i-1}), e_i), empty when M_{i-1} >= e_i.
+__device__ __forceinline__ uint64_t cover_part_lo(const CoverLaunch& c, uint64_t i, uint64_t s) {
+  if (i == 0) return s;
+  const uint64_t m = c.max_end[i - 1];
+  return m > s ? m : s;
+}
+
+// Each match adds the length of its uncovered part to its document's count.  The matches are in start order,
+// so the documents of a warp's lanes do not decrease: a segmented inclusive scan over equal documents leaves
+// each run's sum in its last lane, which alone adds it (one atomic per document per warp).  Every lane takes
+// part in the shuffles, so none returns early.
+__global__ void cover_runs_kernel(CoverLaunch c) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int lane = threadIdx.x & 31;
+  uint64_t doc = ~0ull, part = 0;
+  if (i < c.t.n) {
+    const uint64_t s = c.starts[i], e = s + c.lens[i], lo = cover_part_lo(c, i, s);
+    part = e > lo ? e - lo : 0;
+    doc = doc_of(c.doc_offsets, c.n_docs, c.span_start + s);
+  }
+  for (int o = 1; o < 32; o <<= 1) {
+    const int src = lane >= o ? lane - o : lane;
+    const uint64_t d2 = __shfl_sync(0xffffffffu, doc, src), p2 = __shfl_sync(0xffffffffu, part, src);
+    if (lane >= o && d2 == doc) part += p2;
+  }
+  const uint64_t next = __shfl_sync(0xffffffffu, doc, lane < 31 ? lane + 1 : lane);
+  if (i < c.t.n && part && (lane == 31 || next != doc)) atomicAdd(c.covered + doc, (unsigned long long)part);
+}
+
+// One warp per match writes its uncovered part of the mask: the parts are disjoint, so every covered byte is
+// written once, and a 64 KiB match is 2 K coalesced stores per lane rather than one thread's 64 K.
+__global__ void cover_mask_kernel(CoverLaunch c) {
+  const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint64_t lane = threadIdx.x & 31;
+  if (i >= c.t.n) return;
+  const uint64_t s = c.starts[i], e = s + c.lens[i];
+  uint8_t* m = c.mask + c.span_start;
+  for (uint64_t j = cover_part_lo(c, i, s) + lane; j < e; j += 32) m[j] = 1;
+}
+
 __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
                                      unsigned long long* result) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -561,6 +629,26 @@ cudaError_t launch_count_runs(const CountRunsLaunch& c, cudaStream_t s) {
 
 cudaError_t launch_count_rows(const CountRunsLaunch& c, cudaStream_t s) {
   ACB_LAUNCH(count_rows_kernel, (unsigned)((c.n_docs + 1 + 255) / 256), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_cover_keys(const CoverLaunch& c, cudaStream_t s) {
+  ACB_LAUNCH(cover_keys_kernel, (unsigned)((c.t.n + 255) / 256), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_cover_ends(const CoverLaunch& c, cudaStream_t s) {
+  ACB_LAUNCH(cover_ends_kernel, (unsigned)((c.t.n + 255) / 256), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_cover_runs(const CoverLaunch& c, cudaStream_t s) {
+  ACB_LAUNCH(cover_runs_kernel, (unsigned)((c.t.n + 255) / 256), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_cover_mask(const CoverLaunch& c, cudaStream_t s) {
+  ACB_LAUNCH(cover_mask_kernel, (unsigned)((c.t.n + 7) / 8), 256, 0, s, c);
   return cudaGetLastError();
 }
 

@@ -284,6 +284,26 @@ int acg_pattern_counts_batch_devout(const acg_dfa* dfa, const void* d_hay, uint6
                                     int anchored, int overlapping, uint64_t* d_row_offsets,
                                     uint32_t* d_pids, uint64_t* d_counts, uint64_t cap, uint64_t* nnz);
 
+/* How much of each document of a batch its matches cover.  Let R be the records
+ * acg_find_overlapping_batch (overlapping != 0) or acg_find_iter_batch (overlapping == 0) returns
+ * for the same dfa, haystack, offsets and anchored.  covered[d] (n_docs entries) is the number of
+ * bytes of document d that lie in [start, end) of at least one record of R with doc == d: the
+ * size of the union of the matches, not the sum of their lengths; empty matches cover nothing.
+ * mask (optional, NULL for none) is indexed like hay: for every i in
+ * [doc_offsets[0], doc_offsets[n_docs]) mask[i] = 1 if byte i lies in a match of its document
+ * and 0 otherwise; entries outside that range are left untouched.  The output has a fixed size,
+ * so there is no overflow protocol.  Error codes, their order and the engine are those of the
+ * batch call `overlapping` selects; a NULL covered with n_docs > 0 is ACG_E_INVALID_ARG, and
+ * n_docs == 0 writes nothing.  The union is computed on the device from the matches, without
+ * materialising the records.
+ * _devout: covered and mask are device pointers, doc_offsets as in the other _devout calls. */
+int acg_match_coverage_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                             const uint64_t* doc_offsets, uint64_t n_docs, int anchored, int overlapping,
+                             uint64_t* covered, uint8_t* mask);
+int acg_match_coverage_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_len,
+                                    const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                                    int anchored, int overlapping, uint64_t* d_covered, uint8_t* d_mask);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

@@ -382,6 +382,31 @@ class AhoCorasick {
                                      bool overlapping = false, Anchored a = Anchored::No) const {
     return std::move(try_pattern_counts_batch(haystack, offsets, overlapping, a).unwrap());
   }
+  // How much of each document its matches cover (acg_match_coverage_batch): covered[d] is the number of bytes of
+  // document d inside at least one record of find_overlapping_iter_batch (`overlapping`) or find_iter_batch; with
+  // `with_mask`, mask[i] (one entry per haystack byte) is 1 where byte i lies in a match of its document.
+  struct MatchCoverage {
+    std::vector<uint64_t> covered;  // [n_docs]
+    std::vector<uint8_t> mask;      // [haystack.size()], or empty
+  };
+  Result<MatchCoverage> try_match_coverage_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                                 bool overlapping = false, Anchored a = Anchored::No,
+                                                 bool with_mask = false) const {
+    Result<MatchCoverage> r;
+    if (offsets.empty()) { r.error = ACG_E_INVALID_ARG; return r; }
+    MatchCoverage& c = r.value;
+    c.covered.resize(offsets.size() - 1);
+    if (with_mask) c.mask.assign(haystack.size(), 0);
+    r.error = acg_match_coverage_batch(h_, reinterpret_cast<const uint8_t*>(haystack.data()), 0, haystack.size(),
+                                       offsets.data(), offsets.size() - 1, int(a), int(overlapping), c.covered.data(),
+                                       with_mask ? c.mask.data() : nullptr);
+    if (r.error) c = MatchCoverage{};
+    return r;
+  }
+  MatchCoverage match_coverage_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                     bool overlapping = false, Anchored a = Anchored::No, bool with_mask = false) const {
+    return std::move(try_match_coverage_batch(haystack, offsets, overlapping, a, with_mask).unwrap());
+  }
 
   // replace_all_with / replace_all_with_bytes, :834 / :887 (src/automaton.rs:498-550)
   template <class F>

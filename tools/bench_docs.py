@@ -1,9 +1,10 @@
 #!/usr/bin/env python3
 """Batched search over many documents in one device call (acg_find_overlapping_batch, acg_find_batch,
-acg_pattern_counts_batch).
+acg_pattern_counts_batch, acg_match_coverage_batch).
 
     python tools/bench_docs.py [--hay-gib 4] [--steps 20] [--warmup 5] [--engine 0]
-                               [--call overlapping|find|counts] [--workload cfg2|cfg3] [--out host|device]
+                               [--call overlapping|find|counts|coverage] [--workload cfg2|cfg3] [--out host|device]
+                               [--mask]
 
 cfg 2's automaton and haystack (same seeds as bench.py), device-resident, cut at seeded boundaries into
 documents of log-uniform length in [16 B, 16 KiB] (~1.8 M documents, mean ~2.4 KiB at 4 GiB).  Prints one
@@ -30,6 +31,15 @@ documents: the device records (find_overlapping_iter_batch_torch / find_iter_bat
 torch.unique(doc * P + pid, return_counts=True).  Both give the same matrix (checked).  Device time is measured
 with CUDA events around each whole sequence; the counts call's own scan_ms + order_ms are reported too.
 --out host: the counts go to host memory (pattern_counts_batch_np); device: a CUDA sparse CSR tensor.
+
+--call coverage times match_coverage_batch (the bytes of each document inside at least one match: cfg 2 covers
+with find_overlapping_iter, cfg 3 with find_iter; --mask adds the per-byte mask of the whole haystack) against
+what a caller does without it, alternated step by step on the same documents: the device records
+(find_overlapping_iter_batch_torch / find_iter_batch_torch), sorted by start, torch.cummax of the ends and
+scatter_add of each match's uncovered part per document; for the mask, index_add of +1 at each start and -1 at
+each end, a cumsum over the haystack and > 0.  Both give the same results (checked).  It times three forms in
+one run, whatever --out says: the device-output call (match_coverage_batch_torch, CUDA events and host clock),
+the host-output call (match_coverage_batch_np, host clock) and the records + torch sequence (both clocks).
 """
 import argparse
 import importlib.util
@@ -204,16 +214,112 @@ def bench_counts(args, ac, d_hay, offs, ClockSampler):
         "clocks": clocks.summary()}), flush=True)
 
 
+def coverage_in_torch(r, d_offs, n_docs, n, mask):
+    """(covered, mask or None) of device batch records r (a BatchMatches) with torch operations alone."""
+    import torch
+    s = d_offs[r.doc] + r.start
+    e = d_offs[r.doc] + r.end
+    s, order = torch.sort(s)
+    e, doc = e[order], r.doc[order]
+    m = torch.cummax(e, 0).values
+    prev = torch.cat([torch.zeros(1, dtype=m.dtype, device=m.device), m[:-1]])
+    part = (e - torch.maximum(s, prev)).clamp_(min=0)
+    covered = torch.zeros(n_docs, dtype=torch.int64, device=s.device).scatter_add_(0, doc, part)
+    if not mask:
+        return covered, None
+    d = torch.zeros(n + 1, dtype=torch.int32, device=s.device)
+    one = torch.ones_like(s, dtype=torch.int32)
+    d.index_add_(0, s, one)
+    d.index_add_(0, e, -one)
+    return covered, torch.cumsum(d[:-1], 0, dtype=torch.int32) > 0
+
+
+def bench_coverage(args, ac, d_hay, offs, ClockSampler):
+    """--call coverage: match_coverage_batch (device and host output), and the records + torch path, alternated."""
+    import numpy as np
+    import torch
+    n, n_docs = d_hay.numel(), offs.size - 1
+    overlapping = args.workload == "cfg2"
+    d_offs = torch.from_numpy(offs).cuda()
+    dev_call = lambda: ac.match_coverage_batch_torch((d_hay, d_offs), overlapping=overlapping,  # noqa: E731
+                                                     mask=args.mask)
+    host_call = lambda: ac.match_coverage_batch_np((d_hay, offs), overlapping=overlapping, mask=args.mask)  # noqa
+    records = ac.find_overlapping_iter_batch_torch if overlapping else ac.find_iter_batch_torch
+
+    def records_call():
+        return coverage_in_torch(records((d_hay, d_offs)), d_offs, n_docs, n, args.mask)
+
+    def timed(call):
+        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0 = time.perf_counter()
+        start.record()
+        out = call()
+        end.record()
+        end.synchronize()
+        return out, start.elapsed_time(end), (time.perf_counter() - t0) * 1e3
+
+    for _ in range(args.warmup):
+        dev_call()
+        host_call()
+        records_call()
+    c_dev, c_wall, c_lib, h_wall, r_dev, r_wall = [], [], [], [], [], []
+    with ClockSampler(0) as clocks:
+        for _ in range(args.steps):
+            got, dev_ms, wall_ms = timed(dev_call)
+            st = ac.last_stats()
+            c_dev.append(dev_ms)
+            c_wall.append(wall_ms)
+            c_lib.append(st["scan_ms"] + st["order_ms"])
+            got = None
+            t0 = time.perf_counter()
+            host = host_call()
+            h_wall.append((time.perf_counter() - t0) * 1e3)
+            host = None
+            want, dev_ms, wall_ms = timed(records_call)
+            r_dev.append(dev_ms)
+            r_wall.append(wall_ms)
+            want = None
+    engine = int(st["engine"])
+    got, want = dev_call(), records_call()
+    assert torch.equal(got[0], want[0]), "covered differs from the torch formulation"
+    assert not args.mask or torch.equal(got[1], want[1]), "mask differs from the torch formulation"
+    host = host_call()
+    h_cov = host[0] if args.mask else host
+    assert np.array_equal(h_cov.astype(np.int64), got[0].cpu().numpy()), "host output differs"
+    if args.mask:
+        assert np.array_equal(host[1], got[1].cpu().numpy()), "host mask differs"
+    med = lambda v: float(np.median(v))  # noqa: E731
+    what = "find_overlapping_iter" if overlapping else "find_iter"
+    print(json.dumps({
+        "metric": "match_coverage_device_ms", "value": med(c_dev), "unit": "ms",
+        "steps": args.steps, "warmup": args.warmup,
+        "workload": f"{args.workload}'s automaton and haystack cut into documents of log-uniform length in "
+                    f"[16 B, 16 KiB], the bytes of every document inside its {what} matches"
+                    + (", and the byte mask" if args.mask else ""),
+        "haystack_bytes": n, "documents": n_docs, "mask": args.mask,
+        "engine": {2: "prefilter", 3: "sequential"}.get(engine, engine),
+        "matches": int(st["raw_matches"]), "covered_bytes": int(got[0].sum()),
+        "device_output_call": {"device_ms": med(c_dev), "wall_ms": med(c_wall), "scan_plus_order_ms": med(c_lib),
+                               "scan_ms": float(st["scan_ms"]), "order_ms": float(st["order_ms"])},
+        "host_output_call": {"wall_ms": med(h_wall)},
+        "records_then_torch": {"device_ms": med(r_dev), "wall_ms": med(r_wall)},
+        "timing": "medians; device_ms: CUDA events around each whole sequence; wall_ms: host clock around calls "
+                  "that end in a device synchronise; scan_plus_order_ms: the coverage call's own CUDA events",
+        "check": {"equal_to_torch": True, "host_equal_to_device": True},
+        "clocks": clocks.summary()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--hay-gib", type=float, default=4.0)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--engine", type=int, default=0, help="0 auto, 3 the per-document sequential kernel")
-    ap.add_argument("--call", default="overlapping", choices=["overlapping", "find", "counts"])
+    ap.add_argument("--call", default="overlapping", choices=["overlapping", "find", "counts", "coverage"])
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg3"])
     ap.add_argument("--out", default="host", choices=["host", "device"],
                     help="results to host memory (acg_*_batch) or left in device memory (acg_*_batch_devout)")
+    ap.add_argument("--mask", action="store_true", help="--call coverage: also the per-byte mask")
     args = ap.parse_args()
     if args.call == "overlapping" and args.workload != "cfg2":
         ap.error("find_overlapping_iter needs cfg 2's Standard automaton")
@@ -238,6 +344,8 @@ def main():
         return bench_find(args, ac, d_hay, offs, ClockSampler)
     if args.call == "counts":
         return bench_counts(args, ac, d_hay, offs, ClockSampler)
+    if args.call == "coverage":
+        return bench_coverage(args, ac, d_hay, offs, ClockSampler)
     batch = (d_hay, offs)
     call = ac.find_overlapping_iter_batch_np
     if args.out == "device":
