@@ -165,6 +165,10 @@ def _declare(lib):
                                                     C.POINTER(_u64)]
     lib.acg_match_coverage_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _i, _i, _vp, _vp]
     lib.acg_match_coverage_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _i, _i, _vp, _vp]
+    lib.acg_replace_all_batch.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _vp,
+                                          C.POINTER(_u64)]
+    lib.acg_replace_all_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _vp, _vp, _u64, _vp, _u64, _vp,
+                                                 C.POINTER(_u64)]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -522,6 +526,7 @@ class AhoCorasick:
     def __init__(self, handle):
         self._h = handle
         self._cap_hint = 4096  # output-buffer sizing for the two-call overflow protocol
+        self._replace_ratio = 1.0  # replace_all_batch*: output bytes per input byte that a retry had to make room for
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -975,6 +980,92 @@ class AhoCorasick:
         if rc:
             self._raise(rc)
         return covered, m
+
+    # ---- replace per document (acg_replace_all_batch) ----
+    # replace_all_bytes of every document in one device call: the documents of a batch with the matches of
+    # find_iter_batch replaced by their patterns' replacements, spliced on the device.  The result is a batch in
+    # the (values, offsets) form the batch calls take.
+    def _replacement_table(self, replace_with):
+        """(keepalive, bytes address or None, uint64 offsets [patterns_len() + 1]) of the replacements; ValueError
+        unless there is one per pattern."""
+        reps = self._replacements(replace_with)
+        offs = np.zeros(len(reps) + 1, dtype=np.uint64)
+        if reps:
+            np.cumsum(np.fromiter(map(len, reps), dtype=np.uint64, count=len(reps)), out=offs[1:])
+        data = np.frombuffer(b"".join(reps), dtype=np.uint8)
+        return data, data.ctypes.data if data.size else None, offs
+
+    def _replace_until_it_fits(self, span, alloc, call):
+        """The two-call overflow protocol in output bytes: `call(out, cap, out_len)` on `out = alloc(cap)`, the
+        first guess the span plus an eighth and 4 KiB, scaled by the largest growth a retry of this handle has
+        met.  Returns out[:out_len]."""
+        cnt = _u64()
+        cap = int(span * self._replace_ratio) + span // 8 + 4096
+        while True:
+            out = alloc(cap)
+            rc = call(out, cap, C.byref(cnt))
+            if rc == E_OVERFLOW:
+                need = int(cnt.value)
+                cap = need + need // 8 + 4096
+                self._replace_ratio = max(self._replace_ratio, need / max(span, 1))
+                continue
+            if rc:
+                self._raise(rc)
+            return out[: cnt.value]
+
+    def replace_all_batch_np(self, docs, replace_with):
+        """(values uint8, offsets uint64 [n_docs + 1]): document d with every find_iter match replaced by
+        replace_with[pattern] is values[offsets[d]:offsets[d + 1]], as replace_all_bytes(document) returns it.
+        `docs` as in find_iter_batch_np; one replacement (bytes / str) per pattern."""
+        keep, ptr, n, on_dev, offs = _batch_input(docs)
+        n_docs = offs.size - 1
+        rkeep, rptr, roffs = self._replacement_table(replace_with)
+        out_offsets = np.empty(n_docs + 1, dtype=np.uint64)
+        values = self._replace_until_it_fits(
+            int(offs[-1]) - int(offs[0]), lambda cap: np.empty(cap, dtype=np.uint8),
+            lambda out, cap, cnt: _lib.acg_replace_all_batch(
+                self._h, ptr, on_dev, n, offs.ctypes.data, n_docs, rptr, roffs.ctypes.data, roffs.size - 1,
+                out.ctypes.data, cap, out_offsets.ctypes.data, cnt))
+        return values, out_offsets
+
+    def replace_all_batch(self, docs, replace_with):
+        """replace_all_bytes of every document: one bytes object per document."""
+        values, offs = self.replace_all_batch_np(docs, replace_with)
+        b, o = values.tobytes(), offs.tolist()
+        return [b[o[d]:o[d + 1]] for d in range(len(o) - 1)]
+
+    def replace_all_batch_devout(self, d_hay_ptr, hay_len, offsets, replace_with, out_ptr, cap, out_offsets_ptr,
+                                 n_docs=None):
+        """The replaced documents into device memory: the bytes at out_ptr (cap bytes of room) and their offsets,
+        [n_docs + 1] uint64, at out_offsets_ptr.  Returns the output length; raises OverflowError(needed) if cap
+        is too small (nothing is written then)."""
+        keep, optr, n_docs, on_dev = _devout_offsets(offsets, n_docs)
+        rkeep, rptr, roffs = self._replacement_table(replace_with)
+        cnt = _u64()
+        rc = _lib.acg_replace_all_batch_devout(self._h, d_hay_ptr, hay_len, optr, on_dev, n_docs, rptr,
+                                               roffs.ctypes.data, roffs.size - 1, out_ptr, cap, out_offsets_ptr,
+                                               C.byref(cnt))
+        if rc == E_OVERFLOW:
+            raise OverflowError(int(cnt.value))
+        if rc:
+            self._raise(rc)
+        return int(cnt.value)
+
+    def replace_all_batch_torch(self, docs, replace_with):
+        """(values, CUDA uint8; offsets, CUDA int64 [n_docs + 1]) on the values' device: the replaced documents as
+        a batch.  `docs` as in find_iter_batch_torch."""
+        import torch
+        values, keep, optr, n_docs, on_dev = _torch_batch(docs)
+        dev = values.device
+        rkeep, rptr, roffs = self._replacement_table(replace_with)
+        span = values.numel() if on_dev else int(keep[-1]) - int(keep[0])
+        out_offsets = torch.empty(n_docs + 1, dtype=torch.int64, device=dev)
+        out = self._replace_until_it_fits(
+            span, lambda cap: torch.empty(cap, dtype=torch.uint8, device=dev),
+            lambda out, cap, cnt: _lib.acg_replace_all_batch_devout(
+                self._h, values.data_ptr(), values.numel(), optr, on_dev, n_docs, rptr, roffs.ctypes.data,
+                roffs.size - 1, out.data_ptr(), cap, out_offsets.data_ptr(), cnt))
+        return out, out_offsets
 
     # ---- replace / stream: host-side glue over find_iter, as in the reference -------------------
     @staticmethod

@@ -92,7 +92,8 @@ struct Workspace {
   uint64_t tuple_cap() const { return d_keys[0].cap; }
   DevBuf<unsigned long long> d_counter;
   PinnedBuf<unsigned long long> h_counter;
-  DevBuf<uint8_t> d_temp;  // CUB temporary storage (cub_call): a search's CUB calls run in order on `stream`
+  DevBuf<uint8_t> d_temp;  // CUB temporary storage (cub_call): a search's CUB calls run in order on `stream`;
+                           // after the last of them, the replace splice's tile index
   DevBuf<uint8_t> d_hay;  // staging of host haystacks
   DevBuf<uint64_t> d_scratch;  // chain resolution: end offsets / prefix max
   DevBuf<uint8_t> d_flags;
@@ -106,6 +107,9 @@ struct Workspace {
   DevBuf<uint64_t> d_doc_offs;
   DevBuf<unsigned long long> d_doc_counts, d_doc_incl;
   DevBuf<uint8_t> d_doc_flags;
+  // replace of a batch: the replacement table (offsets, then the bytes) and a host-output call's output
+  DevBuf<uint64_t> d_rep;
+  DevBuf<uint8_t> d_out;
 };
 
 }  // namespace
@@ -1528,33 +1532,33 @@ struct BatchCoverage {
   uint8_t* mask;      // indexed like the haystack, or nullptr
 };
 
-// The mask of [lo, hi), written on the device at d_mask + lo, copied to the host array h_mask + lo: in one copy
-// when that is page-locked, else chunk by chunk through the workspace's staging ring (two page-locked buffers of
-// one pipeline chunk), each chunk's copy to the caller overlapping the next one's transfer.
-int copy_mask_out(const acg_dfa* a, const uint8_t* d_mask, uint8_t* h_mask, uint64_t lo, uint64_t hi) {
+// n bytes from the device at `src` to the host at `dst`: in one copy when `dst` is page-locked, else chunk by chunk
+// through the workspace's staging ring (two page-locked buffers of one pipeline chunk), each chunk's copy to the
+// caller overlapping the next one's transfer.
+int copy_to_host(const acg_dfa* a, uint8_t* dst, const uint8_t* src, uint64_t n) {
   Workspace& w = cur_ws();
-  if (!is_pageable_host(h_mask + lo)) {
-    CK(cudaMemcpyAsync(h_mask + lo, d_mask + lo, hi - lo, cudaMemcpyDeviceToHost, w.stream));
+  if (!is_pageable_host(dst)) {
+    CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, w.stream));
     CK(cudaStreamSynchronize(w.stream));
     return ACG_OK;
   }
-  const uint64_t chunk = std::min<uint64_t>(a->pipeline_chunk, hi - lo);
+  const uint64_t chunk = std::min<uint64_t>(a->pipeline_chunk, n);
   int rc = reserve_stage(w, chunk);
   if (rc) return rc;
   uint64_t at[2] = {0, 0}, len[2] = {0, 0};
   auto drain = [&](int i) -> int {
     if (!len[i]) return ACG_OK;
     CK(cudaEventSynchronize(w.stage_ev[i]));
-    CopyPool::get().copy(h_mask + at[i], w.h_stage[i], size_t(len[i]));
+    CopyPool::get().copy(dst + at[i], w.h_stage[i], size_t(len[i]));
     len[i] = 0;
     return ACG_OK;
   };
   int i = 0;
-  for (uint64_t c0 = lo; c0 < hi; c0 += chunk, i ^= 1) {
+  for (uint64_t c0 = 0; c0 < n; c0 += chunk, i ^= 1) {
     if ((rc = drain(i))) return rc;
     at[i] = c0;
-    len[i] = std::min(chunk, hi - c0);
-    CK(cudaMemcpyAsync(w.h_stage[i], d_mask + c0, len[i], cudaMemcpyDeviceToHost, w.stream));
+    len[i] = std::min(chunk, n - c0);
+    CK(cudaMemcpyAsync(w.h_stage[i], src + c0, len[i], cudaMemcpyDeviceToHost, w.stream));
     CK(cudaEventRecord(w.stage_ev[i], w.stream));
   }
   if ((rc = drain(i))) return rc;  // the older chunk first
@@ -1631,7 +1635,7 @@ int cover_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, int
   if ((rc = reserve_rec(w, (n_docs + 2) / 3))) return rc;  // 3 words per record: room for n_docs words
   CK(cudaEventRecord(w.ev0, w.stream));
   CK(cudaMemcpyAsync(w.h_rec, c.covered, n_docs * 8, cudaMemcpyDeviceToHost, w.stream));
-  if (cv.mask && (rc = copy_mask_out(a, c.mask, cv.mask, span_start, span_end))) return rc;
+  if (cv.mask && (rc = copy_to_host(a, cv.mask + span_start, c.mask + span_start, span_end - span_start))) return rc;
   CK(cudaEventRecord(w.ev1, w.stream));
   CK(cudaStreamSynchronize(w.stream));
   cudaEventElapsedTime(&ms, w.ev0, w.ev1);
@@ -1641,20 +1645,136 @@ int cover_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, int
   return ACG_OK;
 }
 
+// acg_replace_all_batch(_devout): instead of the records of a find_iter batch, the documents with every match
+// replaced (the output arrays in host or device memory, as the call's other outputs; the table in host memory).
+struct BatchReplace {
+  const uint8_t* rep_bytes;
+  const uint64_t* rep_offsets;  // [n_reps + 1]
+  uint64_t n_reps;
+  uint8_t* out;                 // [cap]
+  uint64_t* out_offsets;        // [n_docs + 1]
+};
+
+// One replacement per pattern, with offsets that do not decrease and bytes behind them (the reference asserts the
+// count, src/automaton.rs:443-448).
+bool replacements_ok(const acg_dfa* a, const BatchReplace& rp) {
+  if (!rp.rep_offsets || rp.n_reps != a->h.pattern_lens.size()) return false;
+  for (uint64_t i = 0; i < rp.n_reps; ++i)
+    if (rp.rep_offsets[i + 1] < rp.rep_offsets[i]) return false;
+  return rp.rep_bytes || rp.rep_offsets[rp.n_reps] == rp.rep_offsets[0];
+}
+
+// The n find_iter matches of a batch -- the tuples `t` of the prefilter engine, in start order after the chain, or
+// (t.keys == nullptr) the records the sequential engine left at w.d_rec -- spliced with their replacements into
+// the output (ReplaceLaunch, acb_device.cuh).  `d_in`: the input at span_start, still being read.  Scratch: a_i
+// and e_i in the tuple buffers' keys, pids and documents in their pids, the deltas and their sum in w.d_scratch,
+// the tile index in w.d_temp.  Host output: the bytes in w.d_out and out_offsets in w.d_rec, copied to the caller
+// from there.  *out_len > cap: ACG_E_OVERFLOW, nothing written.
+int replace_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, int mode, uint64_t span_start,
+                    uint64_t span_end, const uint8_t* d_in, const uint64_t* d_offs, uint64_t n_docs,
+                    const BatchReplace& rp, bool dev_out, uint64_t cap, uint64_t* out_len) {
+  Workspace& w = cur_ws();
+  const uint64_t n = t.n, nd1 = n_docs + 1, n_reps = rp.n_reps;
+  const uint64_t rep_total = rp.rep_offsets[n_reps] - rp.rep_offsets[0];
+  int rc;
+  float ms = 0;
+  // the time between ev2 and ev3, to order_ms
+  auto lap = [&]() -> int {
+    CK(cudaEventRecord(w.ev3, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+    w.stats.order_ms += ms;
+    return ACG_OK;
+  };
+  if ((rc = w.d_rep.reserve(n_reps + 1 + (rep_total + 7) / 8))) return rc;
+  CK(cudaMemcpyAsync(w.d_rep, rp.rep_offsets, (n_reps + 1) * 8, cudaMemcpyHostToDevice, w.stream));
+  if (rep_total)
+    CK(cudaMemcpyAsync(w.d_rep + n_reps + 1, rp.rep_bytes + rp.rep_offsets[0], rep_total, cudaMemcpyHostToDevice,
+                       w.stream));
+  acb::ReplaceLaunch r{};
+  r.t = t;
+  r.rec = t.keys ? nullptr : w.d_rec.p;
+  r.mode = mode;
+  r.span_start = span_start;
+  r.doc_offsets = d_offs;
+  r.n_docs = n_docs;
+  r.rep_offsets = w.d_rep;
+  r.rep_bytes = reinterpret_cast<const uint8_t*>(w.d_rep + n_reps + 1);
+  r.in = d_in;
+  uint64_t total = span_end - span_start;
+  CK(cudaEventRecord(w.ev2, w.stream));
+  if (n) {
+    // tuples in buffer b: a_i and pids into the other one, e_i and documents over the tuples; records: 0 and 1
+    const int b = t.keys ? sorted_buf : 1;
+    if (!t.keys && (rc = reserve_tuples(w, std::max<uint64_t>(n, w.tuple_cap())))) return rc;
+    if ((rc = reserve_all(std::max<uint64_t>(n, 1 << 16), w.d_scratch, w.d_flags))) return rc;
+    r.a = w.d_keys[1 - b];
+    r.pids = w.d_pids[1 - b];
+    r.e = w.d_keys[b];
+    r.docs = w.d_pids[b];
+    r.incl = reinterpret_cast<unsigned long long*>(w.d_scratch.p);
+    CK(acb::launch_replace_keys(r, w.stream));
+    if ((rc = cub_call(w, [&](void* tmp, size_t& tb) {
+           return acb::inclusive_sum_u64(tmp, tb, r.incl, r.incl, n, w.stream);
+         })))
+      return rc;
+    CK(cudaMemcpyAsync(w.h_counter, r.incl + n - 1, 8, cudaMemcpyDeviceToHost, w.stream));
+    if ((rc = lap())) return rc;
+    w.stats.launches += 2;
+    total += w.h_counter[0];  // the sum of the length changes, mod 2^64: the output is never shorter than 0
+  }
+  *out_len = total;
+  if (total > cap) return ACG_E_OVERFLOW;
+  r.out_len = total;
+  if (dev_out) {
+    r.out = rp.out;
+    r.out_offsets = rp.out_offsets;
+  } else {
+    if ((rc = w.d_out.reserve(std::max<uint64_t>(total, 1 << 20)))) return rc;
+    if ((rc = reserve_rec(w, (nd1 + 2) / 3))) return rc;  // 3 words per record: room for nd1 words
+    r.out = w.d_out;
+    r.out_offsets = w.d_rec;
+  }
+  const uint64_t n_tiles = total ? acb::replace_splice_tiles(r.out, total) : 0;
+  if ((rc = w.d_temp.reserve(std::max<uint64_t>((n_tiles + 1) * 8, 16)))) return rc;
+  r.tile_first = reinterpret_cast<int64_t*>(w.d_temp.p);
+  CK(cudaEventRecord(w.ev2, w.stream));
+  CK(acb::launch_replace_rows(r, w.stream));
+  w.stats.launches += 1;
+  if (total) {
+    CK(acb::launch_replace_splice(r, w.stream));
+    w.stats.launches += 2;
+  }
+  if ((rc = lap())) return rc;
+  if (dev_out) return ACG_OK;
+  CK(cudaEventRecord(w.ev0, w.stream));
+  CK(cudaMemcpyAsync(w.h_rec, r.out_offsets, nd1 * 8, cudaMemcpyDeviceToHost, w.stream));
+  if (total && (rc = copy_to_host(a, rp.out, r.out, total))) return rc;
+  CK(cudaEventRecord(w.ev1, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+  w.stats.d2h_ms += ms;
+  CopyPool::get().copy(reinterpret_cast<uint8_t*>(rp.out_offsets), reinterpret_cast<const uint8_t*>(w.h_rec.p),
+                       nd1 * 8);
+  return ACG_OK;
+}
+
 // acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch / acg_find_batch (include/acb200.h), and
-// with `co` acg_pattern_counts_batch or with `cv` acg_match_coverage_batch (what: kBatchFindIter or
-// kBatchOverlapping, the records they aggregate; `cap` and `n_out` are those of the counts).  is_match and find
-// give one result per document: flags[n_docs] (find: found) and, for find, out[n_docs].
+// with `co` acg_pattern_counts_batch, with `cv` acg_match_coverage_batch (what: kBatchFindIter or
+// kBatchOverlapping, the records they aggregate; `cap` and `n_out` are those of the counts) or with `rp`
+// acg_replace_all_batch (kBatchFindIter; `cap` and `n_out` in output bytes).  is_match and find give one result
+// per document: flags[n_docs] (find: found) and, for find, out[n_docs].
 int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                const uint64_t* offs, uint64_t n_docs, int anchored, acg_match* out, uint64_t cap, uint64_t* n_out,
                uint8_t* flags, int earliest = 0, const BatchDevOut* dv = nullptr, const BatchCounts* co = nullptr,
-               const BatchCoverage* cv = nullptr) {
+               const BatchCoverage* cv = nullptr, const BatchReplace* rp = nullptr) {
   const bool per_doc = what == kBatchIsMatch || what == kBatchFind;
   if (!a || !offs || (per_doc ? n_docs && (!flags || (what == kBatchFind && !out)) : !n_out))
     return ACG_E_INVALID_ARG;
-  if (cv ? n_docs && !cv->covered
-         : co ? !co->row_offsets || ((!co->pids || !co->counts) && cap)
-              : dv && !per_doc && (!dv->match_offsets || (!out && cap)))
+  if (rp ? !rp->out_offsets || (!rp->out && cap) || !replacements_ok(a, *rp)
+         : cv ? n_docs && !cv->covered
+              : co ? !co->row_offsets || ((!co->pids || !co->counts) && cap)
+                   : dv && !per_doc && (!dv->match_offsets || (!out && cap)))
     return ACG_E_INVALID_ARG;
   if (n_out) *n_out = 0;
   if (n_docs >= (1ull << 32)) return ACG_E_INVALID_ARG;
@@ -1676,6 +1796,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if (!a->on_device) return ACG_E_NO_DEVICE;
   if (n_docs == 0 && !dv) {
     if (co) co->row_offsets[0] = 0;
+    if (rp) rp->out_offsets[0] = 0;
     return ACG_OK;
   }
   earliest = find_earliest(a, anchored, earliest);
@@ -1701,7 +1822,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   uint64_t* const d_index = dv ? dv->match_offsets : reinterpret_cast<uint64_t*>(d_counts);
   uint64_t* d_rec = nullptr;
   uint64_t n_rec = 0;
-  const bool aggregated = co || cv;
+  const bool aggregated = co || cv || rp;
   auto records = [&](uint64_t n) -> int {
     const bool to_caller = dv && !aggregated;
     if (!aggregated && n > cap) return ACG_E_OVERFLOW;
@@ -1729,7 +1850,8 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     CK(cudaMemcpyAsync(w.d_doc_offs, offs, nd1 * 8, cudaMemcpyHostToDevice, w.stream));
   }
   if (n_docs == 0) {  // device output: the index of no records
-    if (!per_doc && !cv) CK(cudaMemsetAsync(co ? co->row_offsets : dv->match_offsets, 0, 8, w.stream));
+    if (!per_doc && !cv)
+      CK(cudaMemsetAsync(co ? co->row_offsets : rp ? rp->out_offsets : dv->match_offsets, 0, 8, w.stream));
     CK(cudaStreamSynchronize(w.stream));
     return ACG_OK;
   }
@@ -1802,6 +1924,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
       if (cv)  // find_iter records are in start order; overlapping ones in end order
         return cover_matches(a, recs, 0, 0, what == kBatchFindIter, span_start, span_end, d_offs, n_docs, *cv,
                              dv != nullptr);
+      if (rp)
+        return replace_matches(a, recs, 0, 0, span_start, span_end, pl.base + span_start, d_offs, n_docs, *rp,
+                               dv != nullptr, cap, n_out);
       return count_matches(a, recs, 0, 0, span_start, d_offs, n_docs, *co, dv != nullptr, cap, n_out);
     }
     // the CSR index is the inclusive scan behind a zero
@@ -1852,6 +1977,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if (co)
     return count_matches(a, tuple_list(a, w, r), r.sorted_buf, chain_mode, span_start, d_offs, n_docs, *co,
                          dv != nullptr, cap, n_out);
+  if (rp)  // the chain's matches in start order: the splice's segments follow each other
+    return replace_matches(a, tuple_list(a, w, r), r.sorted_buf, chain_mode, span_start, span_end,
+                           pl.base + span_start, d_offs, n_docs, *rp, dv != nullptr, cap, n_out);
   *n_out = r.n;
   if ((rc = records(r.n))) return rc;
   CK(cudaEventRecord(w.ev2, w.stream));
@@ -2301,6 +2429,25 @@ int acg_match_coverage_batch_devout(const acg_dfa* a, const void* d_hay, uint64_
   uint64_t unused = 0;
   return batch_impl(a, overlapping ? kBatchOverlapping : kBatchFindIter, static_cast<const uint8_t*>(d_hay), true,
                     hay_len, doc_offsets, n_docs, anchored, nullptr, 0, &unused, nullptr, 0, &dv, nullptr, &cv);
+}
+
+int acg_replace_all_batch(const acg_dfa* a, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                          const uint64_t* doc_offsets, uint64_t n_docs, const uint8_t* rep_bytes,
+                          const uint64_t* rep_offsets, uint64_t n_reps, uint8_t* out, uint64_t cap,
+                          uint64_t* out_offsets, uint64_t* out_len) {
+  const BatchReplace rp{rep_bytes, rep_offsets, n_reps, out, out_offsets};
+  return batch_impl(a, kBatchFindIter, hay, hay_on_device != 0, hay_len, doc_offsets, n_docs, 0, nullptr, cap,
+                    out_len, nullptr, 0, nullptr, nullptr, nullptr, &rp);
+}
+int acg_replace_all_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t hay_len, const uint64_t* doc_offsets,
+                                 int offsets_on_device, uint64_t n_docs, const uint8_t* rep_bytes,
+                                 const uint64_t* rep_offsets, uint64_t n_reps, uint8_t* d_out, uint64_t cap,
+                                 uint64_t* d_out_offsets, uint64_t* out_len) {
+  BatchDevOut dv;
+  dv.offsets_on_device = offsets_on_device != 0;
+  const BatchReplace rp{rep_bytes, rep_offsets, n_reps, d_out, d_out_offsets};
+  return batch_impl(a, kBatchFindIter, static_cast<const uint8_t*>(d_hay), true, hay_len, doc_offsets, n_docs, 0,
+                    nullptr, cap, out_len, nullptr, 0, &dv, nullptr, nullptr, &rp);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

@@ -218,6 +218,40 @@ cudaError_t launch_cover_ends(const CoverLaunch& c, cudaStream_t s);
 cudaError_t launch_cover_runs(const CoverLaunch& c, cudaStream_t s);
 cudaError_t launch_cover_mask(const CoverLaunch& c, cudaStream_t s);
 
+// Replace of a batch (acg_replace_all_batch): the n find_iter matches of a batch, in start order, replaced by their
+// patterns' replacements.  Steps: per match i its document, its pid, its end e_i and a_i = e_i - rep_len_i
+// relative to the span, and delta_i = rep_len_i - (e_i - s_i) (launch_replace_keys; u64, two's complement); the
+// inclusive sum incl_i of the deltas (inclusive_sum_u64 in place), whose last entry gives the output length
+// (span bytes + incl_{n-1}); out_offsets (launch_replace_rows); the output bytes (launch_replace_splice).  In the
+// output, replacement i occupies [q_i, e_i + incl_i) with q_i = a_i + incl_i non-decreasing, and every other byte o
+// is input byte o - incl_i of the gap after the last match i with q_i <= o (o itself before the first match).
+struct ReplaceLaunch {
+  TupleList t;                  // prefilter engine: the tuples; t.n is the number of matches either way
+  const uint64_t* rec;          // sequential engine: [n * 3] acg_doc_match records, else nullptr
+  int mode;                     // tuples: key layout as ChainLaunch::mode
+  uint64_t span_start;
+  const uint64_t* doc_offsets;  // [n_docs + 1]
+  uint64_t n_docs;
+  const uint64_t* rep_offsets;  // [patterns_len + 1] as the caller gave them: rep_offsets[0] need not be 0
+  const uint8_t* rep_bytes;     // replacement p is rep_bytes[rep_offsets[p] - rep_offsets[0] ...)
+  uint64_t* a;                  // [n] e_i - rep_len_i, span-relative (mod 2^64)
+  uint64_t* e;                  // [n] e_i, span-relative
+  uint32_t* pids;               // [n]
+  uint32_t* docs;               // [n] non-decreasing
+  unsigned long long* incl;     // [n] delta_i, then their inclusive sum
+  const uint8_t* in;            // the input at span_start
+  uint8_t* out;                 // [out_len]
+  uint64_t out_len;
+  uint64_t* out_offsets;        // [n_docs + 1]
+  int64_t* tile_first;          // [replace_splice_tiles(out, out_len) + 1] scratch of the splice
+};
+cudaError_t launch_replace_keys(const ReplaceLaunch& r, cudaStream_t s);
+cudaError_t launch_replace_rows(const ReplaceLaunch& r, cudaStream_t s);
+// The number of output tiles of the splice (4 KiB each) and its two launches: the first match of every tile, found
+// by one search per tile, then the tiles.  out_len > 0.
+uint64_t replace_splice_tiles(const uint8_t* out, uint64_t out_len);
+cudaError_t launch_replace_splice(const ReplaceLaunch& r, cudaStream_t s);
+
 // Offsets in device memory: result[0] = 1 if some offs[i] > offs[i + 1] or offs[n_docs] > hay_len (left as it
 // was otherwise: the caller clears it), result[1] = offs[0], result[2] = offs[n_docs].
 cudaError_t launch_check_offsets(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,

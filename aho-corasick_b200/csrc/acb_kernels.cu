@@ -17,6 +17,10 @@
 //        cover_ends_kernel        each match's uncovered part counted per document and written
 //        cover_runs_kernel        to the byte mask
 //        cover_mask_kernel
+//        replace_keys_kernel      replace of a batch: per match its document, pid, end and length change,
+//        replace_rows_kernel      the output offsets by document, the first match of every output tile,
+//        replace_tiles_kernel     and the output spliced tile by tile
+//        replace_splice_kernel
 //        check_offsets_kernel     validation of document offsets in device memory
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
@@ -497,6 +501,145 @@ __global__ void cover_mask_kernel(CoverLaunch c) {
   for (uint64_t j = cover_part_lo(c, i, s) + lane; j < e; j += 32) m[j] = 1;
 }
 
+// Replace, step 1 (ReplaceLaunch): match i's document, pid, end, a_i = end - rep_len and delta_i.  On the prefilter
+// engine `e` and `docs` are the tuple buffers being read: each thread reads its own tuple before it writes there.
+__global__ void replace_keys_kernel(ReplaceLaunch r) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= r.t.n) return;
+  uint64_t start, end, doc;
+  uint32_t pid;
+  if (r.rec) {
+    const uint64_t* q = r.rec + i * 3;
+    pid = (uint32_t)q[0];
+    doc = q[0] >> 32;
+    const uint64_t base = r.doc_offsets[doc] - r.span_start;
+    start = base + q[1];
+    end = base + q[2];
+  } else {
+    pid = r.t.pids[i];
+    const MatchSpan m = decode_key(r.t.keys[i], pid, r.mode, r.span_start, r.t.pattern_lens);
+    doc = doc_of(r.doc_offsets, r.n_docs, m.start);  // tuples are never empty: the start is inside the document
+    start = m.start - r.span_start;
+    end = m.end - r.span_start;
+  }
+  const uint64_t rep_len = r.rep_offsets[pid + 1] - r.rep_offsets[pid];
+  r.a[i] = end - rep_len;
+  r.e[i] = end;
+  r.pids[i] = pid;
+  r.docs[i] = (uint32_t)doc;
+  r.incl[i] = rep_len - (end - start);
+}
+
+// One thread per document d <= n_docs: its output starts where its first byte lands, behind the length changes of
+// the matches of the documents before it (those below the first match whose document is >= d).
+__global__ void replace_rows_kernel(ReplaceLaunch r) {
+  const uint64_t d = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (d > r.n_docs) return;
+  uint64_t lo = 0, hi = r.t.n;
+  while (lo < hi) {
+    const uint64_t mid = lo + ((hi - lo) >> 1);
+    if (r.docs[mid] < d) lo = mid + 1; else hi = mid;
+  }
+  r.out_offsets[d] = r.doc_offsets[d] - r.span_start + (lo ? r.incl[lo - 1] : 0);
+}
+
+// The splice writes the output in tiles of kSpliceTile bytes of the output's 16-byte aligned address space: CTA b
+// owns the bytes o with o + mis in [b * kSpliceTile, (b + 1) * kSpliceTile), mis = the output's address mod 16, and
+// each thread one aligned 16-byte chunk of it.
+constexpr int kSpliceThreads = 256;
+constexpr uint64_t kSpliceTile = kSpliceThreads * 16;
+
+__device__ __forceinline__ uint64_t replace_q(const ReplaceLaunch& r, uint64_t i) { return r.a[i] + r.incl[i]; }
+
+// The last match i in [lo, hi) with q_i <= o, or lo - 1 if there is none (q is non-decreasing).
+__device__ __forceinline__ int64_t replace_last_at(const ReplaceLaunch& r, int64_t lo, int64_t hi, uint64_t o) {
+  while (lo < hi) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    if (replace_q(r, mid) <= o) lo = mid + 1; else hi = mid;
+  }
+  return lo - 1;
+}
+
+__device__ __forceinline__ uint64_t splice_tile_start(uint64_t tile, uint64_t mis) {
+  const uint64_t v = tile * kSpliceTile;
+  return v > mis ? v - mis : 0;
+}
+
+// One thread per tile t <= n_tiles: first[t] = the last match whose q is at or before the tile's first byte (-1:
+// none).  The tile's bytes lie in the segments of matches first[t] .. first[t + 1].
+__global__ void replace_tiles_kernel(ReplaceLaunch r, uint64_t n_tiles, uint64_t mis) {
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t > n_tiles) return;
+  r.tile_first[t] = replace_last_at(r, 0, (int64_t)r.t.n, splice_tile_start(t, mis));
+}
+
+// 16 input bytes from any address: the two aligned words that hold them, shifted together.
+__device__ __forceinline__ uint4 load16(const uint8_t* p) {
+  const uintptr_t addr = reinterpret_cast<uintptr_t>(p);
+  const uint4* w = reinterpret_cast<const uint4*>(addr & ~uintptr_t(15));
+  const uint32_t sh = (uint32_t)(addr & 15);
+  const uint4 x = __ldg(w);
+  if (sh == 0) return x;
+  const uint4 y = __ldg(w + 1);  // holds byte p[15]: inside the input
+  const uint32_t v[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
+  const uint32_t k = sh >> 2, bits = (sh & 3) * 8;
+  uint32_t o[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t lo = k == 0 ? v[j] : k == 1 ? v[j + 1] : k == 2 ? v[j + 2] : v[j + 3];
+    const uint32_t hi = k == 0 ? v[j + 1] : k == 1 ? v[j + 2] : k == 2 ? v[j + 3] : v[j + 4];
+    o[j] = __funnelshift_r(lo, hi, bits);
+  }
+  return make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+// Replace, last step: every output byte written once.  A thread finds the segment of its chunk's first byte with
+// one search among the tile's matches, and moves to the next segment with another only where one starts inside
+// its chunk, so the work per tile is bounded by its 4 KiB of output and the logarithm of its number of matches,
+// whatever the lengths of the documents, gaps and replacements.  A chunk inside one gap is one 16-byte copy.
+__global__ void __launch_bounds__(kSpliceThreads) replace_splice_kernel(ReplaceLaunch r, uint64_t mis) {
+  const uint64_t v = (uint64_t)blockIdx.x * kSpliceTile + threadIdx.x * 16;
+  const uint64_t o = v > mis ? v - mis : 0;
+  const uint64_t o_end = v + 16 - mis < r.out_len ? v + 16 - mis : r.out_len;
+  if (o >= o_end) return;
+  const int64_t f = r.tile_first[blockIdx.x];
+  const int64_t lo = f > 0 ? f : 0, hi = r.tile_first[blockIdx.x + 1] + 1;
+  int64_t i = replace_last_at(r, lo, hi, o);
+  // the segment of match i: its replacement [rep_lo, rep_hi), then the gap up to next_q, input byte o - inc
+  uint64_t inc = 0, rep_lo = 0, rep_hi = 0, rep_at = 0, next_q = ~0ull;
+  auto enter = [&]() {
+    if (i >= 0) {
+      inc = r.incl[i];
+      rep_lo = r.a[i] + inc;
+      rep_hi = r.e[i] + inc;
+      if (rep_hi > rep_lo) rep_at = r.rep_offsets[r.pids[i]] - r.rep_offsets[0];
+    }
+    next_q = i + 1 < hi ? replace_q(r, i + 1) : ~0ull;
+  };
+  enter();
+  uint8_t* dst = r.out + o;
+  const uint64_t n = o_end - o;
+  if (n == 16 && o >= rep_hi && o + 16 <= next_q) {
+    *reinterpret_cast<uint4*>(dst) = load16(r.in + (o - inc));
+    return;
+  }
+  uint64_t w0 = 0, w1 = 0;
+  for (uint64_t j = 0; j < n; ++j) {
+    const uint64_t p = o + j;
+    if (p >= next_q) {
+      i = replace_last_at(r, i + 1, hi, p);
+      enter();
+    }
+    const uint64_t b = p < rep_hi ? r.rep_bytes[rep_at + (p - rep_lo)] : r.in[p - inc];
+    if (j < 8) w0 |= b << (8 * j); else w1 |= b << (8 * (j - 8));
+  }
+  if (n == 16) {
+    *reinterpret_cast<uint4*>(dst) = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
+  } else {
+    for (uint64_t j = 0; j < n; ++j) dst[j] = (uint8_t)((j < 8 ? w0 >> (8 * j) : w1 >> (8 * (j - 8))) & 0xFF);
+  }
+}
+
 __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
                                      unsigned long long* result) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -649,6 +792,27 @@ cudaError_t launch_cover_runs(const CoverLaunch& c, cudaStream_t s) {
 
 cudaError_t launch_cover_mask(const CoverLaunch& c, cudaStream_t s) {
   ACB_LAUNCH(cover_mask_kernel, (unsigned)((c.t.n + 7) / 8), 256, 0, s, c);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_replace_keys(const ReplaceLaunch& r, cudaStream_t s) {
+  ACB_LAUNCH(replace_keys_kernel, (unsigned)((r.t.n + 255) / 256), 256, 0, s, r);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_replace_rows(const ReplaceLaunch& r, cudaStream_t s) {
+  ACB_LAUNCH(replace_rows_kernel, (unsigned)((r.n_docs + 1 + 255) / 256), 256, 0, s, r);
+  return cudaGetLastError();
+}
+
+uint64_t replace_splice_tiles(const uint8_t* out, uint64_t out_len) {
+  return ((reinterpret_cast<uintptr_t>(out) & 15) + out_len + kSpliceTile - 1) / kSpliceTile;
+}
+
+cudaError_t launch_replace_splice(const ReplaceLaunch& r, cudaStream_t s) {
+  const uint64_t mis = reinterpret_cast<uintptr_t>(r.out) & 15, n_tiles = replace_splice_tiles(r.out, r.out_len);
+  ACB_LAUNCH(replace_tiles_kernel, (unsigned)((n_tiles + 1 + 255) / 256), 256, 0, s, r, n_tiles, mis);
+  ACB_LAUNCH(replace_splice_kernel, (unsigned)n_tiles, kSpliceThreads, 0, s, r, mis);
   return cudaGetLastError();
 }
 

@@ -304,6 +304,36 @@ int acg_match_coverage_batch_devout(const acg_dfa* dfa, const void* d_hay, uint6
                                     const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
                                     int anchored, int overlapping, uint64_t* d_covered, uint8_t* d_mask);
 
+/* replace_all_bytes of every document of a batch.  Let R be the records acg_find_iter_batch
+ * returns for the same dfa, haystack and offsets with anchored = 0.  Document d's result is
+ * document d with every record of R of that document replaced by its pattern's replacement, in
+ * order, as the reference's try_replace_all_bytes builds it: the bytes before the first match,
+ * the replacement, the bytes between the first and the second match, ..., the bytes after the
+ * last one.  Empty matches insert their replacement; replacements are not searched again.
+ * Replacement i (n_reps == patterns_len entries) is rep_bytes[rep_offsets[i] .. rep_offsets[i + 1]);
+ * the table is in host memory for both calls.  n_reps != patterns_len, decreasing rep_offsets, a
+ * NULL rep_offsets or a NULL rep_bytes with replacement bytes give ACG_E_INVALID_ARG.
+ * The results are in the CSR form every batch call takes: document d's bytes are
+ * out[out_offsets[d] .. out_offsets[d + 1]), out_offsets has n_docs + 1 entries, out_offsets[0] = 0
+ * and *out_len = out_offsets[n_docs].  If *out_len > cap the call returns ACG_E_OVERFLOW with the
+ * required size in *out_len and writes neither out nor out_offsets; cap == 0 with a NULL out is a
+ * size query.  A NULL out with cap > 0, a NULL out_offsets or a NULL out_len is ACG_E_INVALID_ARG.
+ * Otherwise the error codes, their order and the engine are those of acg_find_iter_batch with
+ * anchored = 0 (an automaton built with ACG_START_ANCHORED gives ACG_E_INVALID_INPUT_UNANCHORED).
+ * n_docs == 0 writes out_offsets[0] = 0 and *out_len = 0.  The output is spliced on the device
+ * from the matches, without materialising the records.
+ * out must not overlap the haystack: the input is still read while the output is written.
+ * _devout: out and out_offsets are device pointers, doc_offsets as in the other _devout calls;
+ * out_len is a host pointer. */
+int acg_replace_all_batch(const acg_dfa* dfa, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                          const uint64_t* doc_offsets, uint64_t n_docs,
+                          const uint8_t* rep_bytes, const uint64_t* rep_offsets, uint64_t n_reps,
+                          uint8_t* out, uint64_t cap, uint64_t* out_offsets, uint64_t* out_len);
+int acg_replace_all_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t hay_len,
+                                 const uint64_t* doc_offsets, int offsets_on_device, uint64_t n_docs,
+                                 const uint8_t* rep_bytes, const uint64_t* rep_offsets, uint64_t n_reps,
+                                 uint8_t* d_out, uint64_t cap, uint64_t* d_out_offsets, uint64_t* out_len);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

@@ -407,6 +407,45 @@ class AhoCorasick {
                                      bool overlapping = false, Anchored a = Anchored::No, bool with_mask = false) const {
     return std::move(try_match_coverage_batch(haystack, offsets, overlapping, a, with_mask).unwrap());
   }
+  // replace_all_bytes of every document (acg_replace_all_batch): the documents with their find_iter matches
+  // replaced by replacements[pattern], spliced on the device, as a batch: document d's result is
+  // bytes[offsets[d] .. offsets[d + 1]).  One replacement per pattern, or ACG_E_INVALID_ARG.
+  struct ReplacedBatch {
+    std::string bytes;
+    std::vector<uint64_t> offsets;  // [n_docs + 1]
+  };
+  template <class Replacements>
+  Result<ReplacedBatch> try_replace_all_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                              const Replacements& replacements) const {
+    Result<ReplacedBatch> r;
+    if (offsets.empty()) { r.error = ACG_E_INVALID_ARG; return r; }
+    std::string table;
+    std::vector<uint64_t> at{0};
+    for (const auto& x : replacements) {
+      table.append(std::string_view(x));
+      at.push_back(table.size());
+    }
+    ReplacedBatch& b = r.value;
+    b.offsets.resize(offsets.size());
+    const uint64_t span = offsets.back() >= offsets.front() ? offsets.back() - offsets.front() : 0;
+    uint64_t need = 0;
+    for (uint64_t cap = span + span / 8 + 4096;; cap = need) {
+      b.bytes.resize(cap);
+      r.error = acg_replace_all_batch(h_, reinterpret_cast<const uint8_t*>(haystack.data()), 0, haystack.size(),
+                                      offsets.data(), offsets.size() - 1,
+                                      reinterpret_cast<const uint8_t*>(table.data()), at.data(), at.size() - 1,
+                                      reinterpret_cast<uint8_t*>(b.bytes.data()), cap, b.offsets.data(), &need);
+      if (r.error != ACG_E_OVERFLOW) break;  // two-call protocol: need is the required size
+    }
+    if (r.error) b = ReplacedBatch{};
+    else b.bytes.resize(need);
+    return r;
+  }
+  template <class Replacements>
+  ReplacedBatch replace_all_batch(std::string_view haystack, const std::vector<uint64_t>& offsets,
+                                  const Replacements& replacements) const {
+    return std::move(try_replace_all_batch(haystack, offsets, replacements).unwrap());
+  }
 
   // replace_all_with / replace_all_with_bytes, :834 / :887 (src/automaton.rs:498-550)
   template <class F>

@@ -1,9 +1,10 @@
 #!/usr/bin/env python3
 """Batched search over many documents in one device call (acg_find_overlapping_batch, acg_find_batch,
-acg_pattern_counts_batch, acg_match_coverage_batch).
+acg_pattern_counts_batch, acg_match_coverage_batch, acg_replace_all_batch).
 
     python tools/bench_docs.py [--hay-gib 4] [--steps 20] [--warmup 5] [--engine 0]
-                               [--call overlapping|find|counts|coverage] [--workload cfg2|cfg3] [--out host|device]
+                               [--call overlapping|find|counts|coverage|replace] [--workload cfg2|cfg3]
+                               [--out host|device]
                                [--mask]
 
 cfg 2's automaton and haystack (same seeds as bench.py), device-resident, cut at seeded boundaries into
@@ -40,6 +41,16 @@ scatter_add of each match's uncovered part per document; for the mask, index_add
 each end, a cumsum over the haystack and > 0.  Both give the same results (checked).  It times three forms in
 one run, whatever --out says: the device-output call (match_coverage_batch_torch, CUDA events and host clock),
 the host-output call (match_coverage_batch_np, host clock) and the records + torch sequence (both clocks).
+
+--call replace times replace_all_batch (every document with its find_iter matches replaced: cfg 2 Standard, cfg 3
+leftmost-first) with a seeded table that mixes deletions, same-length and longer replacements, against what a
+caller does without it, alternated step by step on the same documents: the device records (find_iter_batch_torch)
+spliced in torch -- the exclusive cumsum D of the length changes, q = start + D, and per output byte a
+searchsorted over q, in windows of 512 MiB of output.  Both give the same bytes (checked).  It times, in one run,
+the device-output call (replace_all_batch_torch), the host-output call (replace_all_batch_np), the records + torch
+splice, and a device-to-device cudaMemcpy of the span as the copy baseline of the same session; torch.profiler
+gives the splice kernel's own time.  The call-overhead check runs 10 000 replace_all_bytes calls against one batch
+call over the same documents (same bytes).
 """
 import argparse
 import importlib.util
@@ -309,13 +320,156 @@ def bench_coverage(args, ac, d_hay, offs, ClockSampler):
         "clocks": clocks.summary()}), flush=True)
 
 
+def replacement_table(pats, seed=0xBE4C):
+    """A seeded replacement per pattern: a deletion, a same-length filler or a longer tag, a third each."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    return [(b"", b"#" * len(p), b"<%d:" % i + p + b">")[int(rng.integers(0, 3))] for i, p in enumerate(pats)]
+
+
+def replace_in_torch(r, d_hay, d_offs, reps_dev, window=512 << 20):
+    """(values, offsets) of device batch records r (a BatchMatches) spliced with torch operations alone."""
+    import torch
+    rep_len, rep_at, rep_data = reps_dev
+    dev = d_hay.device
+    lo = int(d_offs[0])
+    s = d_offs[r.doc] - lo + r.start
+    delta = rep_len[r.pid] - (r.end - r.start)
+    incl = torch.cumsum(delta, 0)
+    q = s + incl - delta
+    offsets = d_offs - lo + torch.cat([torch.zeros(1, dtype=torch.int64, device=dev), incl])[r.offsets]
+    n_out = int(offsets[-1])
+    out = torch.empty(n_out, dtype=torch.uint8, device=dev)
+    for w0 in range(0, n_out, window):
+        o = torch.arange(w0, min(n_out, w0 + window), dtype=torch.int64, device=dev)
+        i = torch.searchsorted(q, o, right=True) - 1
+        ok = i >= 0
+        ic = i.clamp(min=0)
+        qi = torch.where(ok, q[ic], 0)
+        pid = r.pid[ic]
+        in_rep = ok & (o < qi + rep_len[pid])
+        src = (lo + o - torch.where(ok, incl[ic], 0)).clamp(max=d_hay.numel() - 1)
+        out[w0:w0 + o.numel()] = torch.where(in_rep, rep_data[(rep_at[pid] + o - qi).clamp(0, rep_data.numel() - 1)],
+                                             d_hay[src])
+        del o, i, ok, ic, qi, pid, in_rep, src
+    return out, offsets
+
+
+def bench_replace(args, ac, d_hay, offs, ClockSampler):
+    """--call replace: replace_all_batch (device and host output), the records + torch splice and a D2D copy of the
+    span, alternated step by step; the splice kernel's time from torch.profiler; the call-overhead check."""
+    import numpy as np
+    import torch
+    from aho_corasick_b200 import workload as W
+    n, n_docs = d_hay.numel(), offs.size - 1
+    reps = replacement_table(W.config_patterns(args.workload))
+    d_offs = torch.from_numpy(offs).cuda()
+    rep_len = torch.tensor([len(x) for x in reps], dtype=torch.int64, device="cuda")
+    reps_dev = (rep_len, torch.cumsum(rep_len, 0) - rep_len,
+                torch.frombuffer(bytearray(b"".join(reps) or b"\0"), dtype=torch.uint8).cuda())
+    dev_call = lambda: ac.replace_all_batch_torch((d_hay, d_offs), reps)  # noqa: E731
+    host_call = lambda: ac.replace_all_batch_np((d_hay, offs), reps)  # noqa: E731
+    records_call = lambda: replace_in_torch(ac.find_iter_batch_torch((d_hay, d_offs)), d_hay, d_offs, reps_dev)  # noqa
+    span = torch.empty_like(d_hay)
+    copy_call = lambda: span.copy_(d_hay)  # noqa: E731  (one cudaMemcpyAsync device to device)
+
+    def timed(call):
+        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0 = time.perf_counter()
+        start.record()
+        out = call()
+        end.record()
+        end.synchronize()
+        return out, start.elapsed_time(end), (time.perf_counter() - t0) * 1e3
+
+    for _ in range(args.warmup):
+        dev_call()
+        host_call()
+        records_call()
+        copy_call()
+    c_dev, c_wall, c_order, h_wall, r_dev, r_wall, cp_dev = [], [], [], [], [], [], []
+    with ClockSampler(0) as clocks:
+        for _ in range(args.steps):
+            got, dev_ms, wall_ms = timed(dev_call)
+            st = ac.last_stats()
+            c_dev.append(dev_ms)
+            c_wall.append(wall_ms)
+            c_order.append(st["order_ms"])
+            got = None
+            t0 = time.perf_counter()
+            host = host_call()
+            h_wall.append((time.perf_counter() - t0) * 1e3)
+            host = None
+            want, dev_ms, wall_ms = timed(records_call)
+            r_dev.append(dev_ms)
+            r_wall.append(wall_ms)
+            want = None
+            cp_dev.append(timed(copy_call)[1])
+    engine = int(st["engine"])
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        dev_call()
+        torch.cuda.synchronize()
+    splice_us = 0.0
+    for ev in prof.key_averages():
+        if "replace_splice_kernel" in ev.key:
+            splice_us += getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
+    got, want = dev_call(), records_call()
+    assert torch.equal(got[1], want[1]), "offsets differ from the torch splice"
+    assert torch.equal(got[0], want[0]), "bytes differ from the torch splice"
+    n_out = got[0].numel()
+    host = host_call()
+    assert np.array_equal(host[1].astype(np.int64), got[1].cpu().numpy()), "host offsets differ"
+    assert torch.equal(torch.from_numpy(host[0]).cuda(), got[0]), "host bytes differ"
+    want = host = None
+    # call overhead: one replace_all_bytes per document against one batch call, host haystack, same bytes
+    k = min(10_000, n_docs)
+    h = d_hay[: int(offs[k])].cpu().numpy()
+    docs = [h[offs[d]:offs[d + 1]].tobytes() for d in range(k)]
+    for d in docs[:100]:  # warm
+        ac.replace_all_bytes(d, reps)
+    t0 = time.perf_counter()
+    per_doc = [ac.replace_all_bytes(d, reps) for d in docs]
+    per_doc_s = time.perf_counter() - t0
+    ac.replace_all_batch(docs, reps)
+    t0 = time.perf_counter()
+    batch = ac.replace_all_batch(docs, reps)
+    batch_s = time.perf_counter() - t0
+    assert batch == per_doc, "batch call differs from replace_all_bytes"
+    med = lambda v: float(np.median(v))  # noqa: E731
+    splice_ms = splice_us / 1e3
+    print(json.dumps({
+        "metric": "replace_device_ms", "value": med(c_dev), "unit": "ms",
+        "steps": args.steps, "warmup": args.warmup,
+        "workload": f"{args.workload}'s automaton and haystack cut into documents of log-uniform length in "
+                    "[16 B, 16 KiB], every document's find_iter matches replaced from a seeded table of deletions, "
+                    "same-length and longer replacements",
+        "haystack_bytes": n, "documents": n_docs, "output_bytes": n_out,
+        "engine": {2: "prefilter", 3: "sequential"}.get(engine, engine), "matches": int(st["raw_matches"]),
+        "device_output_call": {"device_ms": med(c_dev), "wall_ms": med(c_wall),
+                               "input_gib_per_s": n / GIB / med(c_dev) * 1e3, "scan_ms": float(st["scan_ms"]), "order_ms": med(c_order)},
+        "host_output_call": {"wall_ms": med(h_wall)},
+        "records_then_torch": {"device_ms": med(r_dev), "wall_ms": med(r_wall)},
+        "splice_kernel": {"device_ms": splice_ms, "read_plus_written_gb_per_s": (n + n_out) / 1e6 / splice_ms
+                          if splice_ms else None},
+        "d2d_copy_of_the_span": {"device_ms": med(cp_dev), "read_plus_written_gb_per_s": 2 * n / 1e6 / med(cp_dev)},
+        "timing": "medians; device_ms: CUDA events around each whole sequence; wall_ms: host clock around calls "
+                  "that end in a device synchronise; order_ms: the replace call's own CUDA events after the scan "
+                  "(per-match keys, scan of the length changes, offsets, splice); splice_kernel: torch.profiler",
+        "check": {"equal_to_torch": True, "host_equal_to_device": True},
+        "call_overhead": {"documents": k, "one_replace_all_bytes_per_document_ms": per_doc_s * 1e3,
+                          "one_batch_call_ms": batch_s * 1e3, "same_bytes": True,
+                          "timing": "host clock, host haystack"},
+        "clocks": clocks.summary()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--hay-gib", type=float, default=4.0)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--engine", type=int, default=0, help="0 auto, 3 the per-document sequential kernel")
-    ap.add_argument("--call", default="overlapping", choices=["overlapping", "find", "counts", "coverage"])
+    ap.add_argument("--call", default="overlapping", choices=["overlapping", "find", "counts", "coverage", "replace"])
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg3"])
     ap.add_argument("--out", default="host", choices=["host", "device"],
                     help="results to host memory (acg_*_batch) or left in device memory (acg_*_batch_devout)")
@@ -346,6 +500,8 @@ def main():
         return bench_counts(args, ac, d_hay, offs, ClockSampler)
     if args.call == "coverage":
         return bench_coverage(args, ac, d_hay, offs, ClockSampler)
+    if args.call == "replace":
+        return bench_replace(args, ac, d_hay, offs, ClockSampler)
     batch = (d_hay, offs)
     call = ac.find_overlapping_iter_batch_np
     if args.out == "device":
