@@ -169,6 +169,13 @@ def _declare(lib):
                                           C.POINTER(_u64)]
     lib.acg_replace_all_batch_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _vp, _vp, _u64, _vp, _u64, _vp,
                                                  C.POINTER(_u64)]
+    lib.acg_streams_create.argtypes = [_vp, _u64, _i, C.POINTER(_vp)]
+    lib.acg_streams_free.argtypes = [_vp]
+    lib.acg_streams_free.restype = None
+    lib.acg_streams_reset.argtypes = [_vp, _vp, _u64]
+    lib.acg_streams_positions.argtypes = [_vp, _vp]
+    lib.acg_streams_feed.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _vp, _u64, C.POINTER(_u64)]
+    lib.acg_streams_feed_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _vp, _u64, _vp, C.POINTER(_u64)]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -1177,6 +1184,11 @@ class AhoCorasick:
 
     stream_find_iter = try_stream_find_iter      # :906
 
+    def streams(self, n_streams, overlapping=False):
+        """A set of n_streams byte streams searched on the device as their bytes arrive (acg_streams_*): each
+        feed returns the matches that end in the bytes it brought, with offsets into the whole stream."""
+        return Streams(self, n_streams, overlapping)
+
     def try_stream_replace_all_with(self, rdr, wtr, replace_with, chunk_bytes=64 << 20):
         """`try_stream_replace_all_with`, src/ahocorasick.rs:1807 -> src/automaton.rs:601-636:
         `replace_with(match, matched bytes, wtr)` writes the replacement; text between matches is
@@ -1236,3 +1248,101 @@ class AhoCorasick:
         if rc:
             self._raise(rc)
         return cnt.value, fnv.value, ms.value
+
+
+class Streams:
+    """A stream set (include/acb200.h, acg_streams_*): n_streams streams over one automaton, in find_iter mode
+    (try_find_iter, Standard semantics) or overlapping mode (try_find_overlapping_iter).  A feed takes one chunk per
+    stream -- in any form the batch calls take -- and returns, per stream, the matches of the mode's iterator over
+    everything the stream has received whose end lies in this feed's bytes, offsets absolute within the stream.  A
+    stream's matches over all its feeds, concatenated, are the iterator over its concatenated chunks.  One call at a
+    time per set.  Create it with AhoCorasick.streams(); the automaton is kept alive by the set."""
+
+    def __init__(self, ac, n_streams, overlapping=False):
+        self._ac = ac
+        self._h = None
+        h = _vp()
+        rc = _lib.acg_streams_create(ac._h, int(n_streams), int(bool(overlapping)), C.byref(h))
+        if rc:
+            ac._raise(rc)
+        self._h = h
+        self.n_streams = int(n_streams)
+        self.overlapping = bool(overlapping)
+
+    def close(self):
+        if self._h and _lib is not None:
+            _lib.acg_streams_free(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def _check(self, n_chunks):
+        if not self._h:
+            raise ValueError("the stream set is closed")
+        if n_chunks != self.n_streams:
+            raise ValueError(f"a feed takes one chunk per stream: {n_chunks} chunks for {self.n_streams} streams")
+
+    def feed_np(self, chunks):
+        """One chunk per stream (a list of bytes / str, or (values, offsets) as the batch calls take): the new
+        matches as a DOC_MATCH_DTYPE array, doc = the stream, ascending stream."""
+        keep, ptr, n, on_dev, offs = _batch_input(chunks)
+        self._check(offs.size - 1)
+        cnt = _u64()
+        return _until_it_fits(
+            self._ac, max(self._ac._cap_hint, 64), lambda cap: np.empty(cap, DOC_MATCH_DTYPE), cnt,
+            lambda out, cap: _lib.acg_streams_feed(self._h, ptr, on_dev, n, offs.ctypes.data, self.n_streams,
+                                                   out.ctypes.data, cap, C.byref(cnt)))
+
+    def feed(self, chunks):
+        """One chunk per stream: one list of Match per stream."""
+        return AhoCorasick._per_doc(self.feed_np(chunks), self.n_streams)
+
+    def feed_torch(self, chunks):
+        """(values, offsets) chunks with values a CUDA torch.uint8 tensor and offsets an int64 CUDA tensor on its
+        device or a host array: the new matches as a BatchMatches of CUDA tensors, indexed by stream."""
+        import torch
+        values, keep, optr, n_chunks, on_dev = _torch_batch(chunks)
+        self._check(n_chunks)
+        match_offsets = torch.empty(n_chunks + 1, dtype=torch.int64, device=values.device)
+        cnt = _u64()
+        r = _until_it_fits(
+            self._ac, self._ac._cap_hint, lambda cap: torch.empty((cap, 3), dtype=torch.int64, device=values.device),
+            cnt, lambda records, cap: _lib.acg_streams_feed_devout(
+                self._h, values.data_ptr(), values.numel(), optr, on_dev, self.n_streams, records.data_ptr(), cap,
+                match_offsets.data_ptr(), C.byref(cnt)))
+        return BatchMatches(r, match_offsets, r[:, 0] & 0xFFFFFFFF, r[:, 0] >> 32, r[:, 1], r[:, 2])
+
+    def reset(self, ids=None):
+        """Restart the given streams (all when ids is None) from zero bytes."""
+        self._check(self.n_streams)
+        if ids is None:
+            rc = _lib.acg_streams_reset(self._h, None, 0)
+        else:
+            a = np.ascontiguousarray(np.asarray(ids, dtype=np.int64).reshape(-1))
+            if (a < 0).any():
+                raise ValueError("stream ids must be non-negative")
+            if a.size == 0:
+                return
+            a = a.astype(np.uint64)
+            rc = _lib.acg_streams_reset(self._h, a.ctypes.data, a.size)
+        if rc:
+            self._ac._raise(rc)
+
+    def positions(self):
+        """The bytes every stream has received: uint64 [n_streams]."""
+        self._check(self.n_streams)
+        pos = np.empty(self.n_streams, dtype=np.uint64)
+        rc = _lib.acg_streams_positions(self._h, pos.ctypes.data)
+        if rc:
+            self._ac._raise(rc)
+        return pos

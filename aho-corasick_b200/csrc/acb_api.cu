@@ -14,6 +14,7 @@
 #include <mutex>
 #include <thread>
 #include <new>
+#include <optional>
 #include <vector>
 
 #include "../../include/acb200.h"
@@ -109,7 +110,10 @@ struct Workspace {
   DevBuf<uint8_t> d_doc_flags;
   // replace of a batch: the replacement table (offsets, then the bytes) and a host-output call's output
   DevBuf<uint64_t> d_rep;
-  DevBuf<uint8_t> d_out;
+  DevBuf<uint8_t> d_out;  // also a host-output stream feed's records
+  // a stream feed: the combined documents tail | chunk, their offsets and the chunk offsets given on the host
+  DevBuf<uint8_t> d_sdocs;
+  DevBuf<uint64_t> d_soffs;
 };
 
 }  // namespace
@@ -145,6 +149,15 @@ struct acg_dfa {
   mutable std::vector<Workspace*> ws_all, ws_free;
   mutable std::condition_variable ws_cv;
   mutable acg_stats last_stats{};  // of the search that finished last (acg_last_stats from another thread)
+};
+
+// A stream set (acg_streams_create): the state of StreamLaunch (acb_device.cuh) on the automaton's device.
+struct acg_streams {
+  const acg_dfa* a = nullptr;
+  uint64_t n = 0, back = 0;
+  bool overlapping = false;
+  uint64_t* d_state = nullptr;  // [2 * n]: pos, then cursor
+  uint8_t* d_tail = nullptr;    // [n * back]
 };
 
 namespace {
@@ -1759,15 +1772,82 @@ int replace_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, i
   return ACG_OK;
 }
 
+// acg_streams_feed(_devout): the batch is the feed's combined documents D in the workspace (offsets on the device,
+// `docs_len` bytes), and its records become the feed's (StreamLaunch, acb_device.cuh).  `out` and `out_index` are
+// the caller's device arrays, or (`out_index` == nullptr) `out` is the caller's host array.
+struct BatchStreams {
+  acb::StreamLaunch launch;  // the set, the chunks and D; the records and outputs are filled in by stream_records
+  uint64_t docs_len;
+  uint64_t* out;
+  uint64_t* out_index;
+};
+
+// The m records of D at `rec` with their index: the ones a previous feed has not returned (overlapping: those that
+// end after their tail), rebased and tagged, then the state of every stream.  ms_to gets the batch's time from ev2
+// to ev3.  *n_out > cap: ACG_E_OVERFLOW, and nothing -- state included -- is written.
+int stream_records(const acg_dfa* a, const BatchStreams& st, const uint64_t* rec, const uint64_t* rec_index,
+                   uint64_t m, uint64_t cap, uint64_t* n_out, float& ms_to) {
+  Workspace& w = cur_ws();
+  float ms = 0;
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+  ms_to += ms;
+  acb::StreamLaunch p = st.launch;
+  p.rec = rec;
+  p.rec_index = rec_index;
+  p.m = m;
+  p.keep = nullptr;
+  uint64_t kept = m;
+  int rc;
+  CK(cudaEventRecord(w.ev2, w.stream));
+  if (p.overlapping && m) {
+    if ((rc = reserve_all(std::max<uint64_t>(m, 1 << 16), w.d_scratch, w.d_flags))) return rc;
+    p.keep = reinterpret_cast<unsigned long long*>(w.d_scratch.p);
+    CK(acb::launch_stream_keep(p, w.stream));
+    if ((rc = cub_call(w, [&](void* tmp, size_t& tb) {
+           return acb::inclusive_sum_u64(tmp, tb, p.keep, p.keep, m, w.stream);
+         })))
+      return rc;
+    CK(cudaMemcpyAsync(w.h_counter, p.keep + m - 1, 8, cudaMemcpyDeviceToHost, w.stream));
+    CK(cudaStreamSynchronize(w.stream));
+    w.stats.launches += 2;
+    kept = w.h_counter[0];
+  }
+  *n_out = kept;
+  if (kept > cap) return ACG_E_OVERFLOW;
+  if (kept && !st.out) return ACG_E_INVALID_ARG;
+  const bool dev_out = st.out_index != nullptr;
+  if (!dev_out && (rc = w.d_out.reserve(std::max<uint64_t>(kept * 24, 1 << 20)))) return rc;
+  p.out = dev_out ? st.out : reinterpret_cast<uint64_t*>(w.d_out.p);
+  p.out_index = st.out_index;
+  CK(acb::launch_stream_records(p, w.stream));
+  CK(acb::launch_stream_state(p, w.stream));
+  CK(cudaEventRecord(w.ev3, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+  w.stats.order_ms += ms;
+  w.stats.launches += 2;
+  if (dev_out || !kept) return ACG_OK;
+  CK(cudaEventRecord(w.ev0, w.stream));
+  if ((rc = copy_to_host(a, reinterpret_cast<uint8_t*>(st.out), w.d_out, kept * 24))) return rc;
+  CK(cudaEventRecord(w.ev1, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+  w.stats.d2h_ms += ms;
+  return ACG_OK;
+}
+
 // acg_find_iter_batch / acg_find_overlapping_batch / acg_is_match_batch / acg_find_batch (include/acb200.h), and
 // with `co` acg_pattern_counts_batch, with `cv` acg_match_coverage_batch (what: kBatchFindIter or
 // kBatchOverlapping, the records they aggregate; `cap` and `n_out` are those of the counts) or with `rp`
 // acg_replace_all_batch (kBatchFindIter; `cap` and `n_out` in output bytes).  is_match and find give one result
-// per document: flags[n_docs] (find: found) and, for find, out[n_docs].
+// per document: flags[n_docs] (find: found) and, for find, out[n_docs].  With `st` a stream feed, which holds the
+// workspace already, searches its combined documents (`hay`, `offs` on the device; `cap` and `n_out` those of the
+// feed's records).
 int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
                const uint64_t* offs, uint64_t n_docs, int anchored, acg_match* out, uint64_t cap, uint64_t* n_out,
                uint8_t* flags, int earliest = 0, const BatchDevOut* dv = nullptr, const BatchCounts* co = nullptr,
-               const BatchCoverage* cv = nullptr, const BatchReplace* rp = nullptr) {
+               const BatchCoverage* cv = nullptr, const BatchReplace* rp = nullptr, const BatchStreams* st = nullptr) {
   const bool per_doc = what == kBatchIsMatch || what == kBatchFind;
   if (!a || !offs || (per_doc ? n_docs && (!flags || (what == kBatchFind && !out)) : !n_out))
     return ACG_E_INVALID_ARG;
@@ -1778,7 +1858,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     return ACG_E_INVALID_ARG;
   if (n_out) *n_out = 0;
   if (n_docs >= (1ull << 32)) return ACG_E_INVALID_ARG;
-  const bool offs_on_device = dv && dv->offsets_on_device;
+  const bool offs_on_device = (dv && dv->offsets_on_device) || st;
   if (offs_on_device) {
     if (reinterpret_cast<uintptr_t>(offs) & 7) return ACG_E_INVALID_ARG;
   } else {
@@ -1804,8 +1884,11 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   if (engine < 0) return engine;
   const bool use_pf = engine == ACG_ENGINE_PREFILTER;
   DeviceGuard guard(a->device);
-  WsLease lease(a);
-  if (lease.rc) return lease.rc;
+  std::optional<WsLease> lease;
+  if (!st) {
+    lease.emplace(a);
+    if (lease->rc) return lease->rc;
+  }
   Workspace& w = cur_ws();
   w.stats.engine = engine;
   const uint64_t nd1 = n_docs + 1;
@@ -1825,15 +1908,19 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   const bool aggregated = co || cv || rp;
   auto records = [&](uint64_t n) -> int {
     const bool to_caller = dv && !aggregated;
-    if (!aggregated && n > cap) return ACG_E_OVERFLOW;
-    if (!aggregated && n && !out) return ACG_E_INVALID_ARG;
+    if (!aggregated && !st && n > cap) return ACG_E_OVERFLOW;
+    if (!aggregated && !st && n && !out) return ACG_E_INVALID_ARG;
     n_rec = n;
     const int e = to_caller ? ACG_OK : reserve_rec(w, n);
     d_rec = to_caller ? reinterpret_cast<uint64_t*>(out) : w.d_rec.p;
     return e;
   };
   if (what == kBatchFind && (rc = records(n_docs))) return rc;
-  if (offs_on_device) {
+  if (st) {  // built by the feed: bounds known to hold
+    span_start = 0;
+    span_end = st->docs_len;
+    d_offs = offs;
+  } else if (offs_on_device) {
     // checked where they are; the span bounds come back with the verdict (placement and the scan plan need them)
     CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
     CK(acb::launch_check_offsets(offs, n_docs, hay_len, w.d_counter, w.stream));
@@ -1932,6 +2019,7 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     // the CSR index is the inclusive scan behind a zero
     CK(cudaMemsetAsync(d_index, 0, 8, w.stream));
     CK(cudaMemcpyAsync(d_index + 1, d_incl, n_docs * 8, cudaMemcpyDeviceToDevice, w.stream));
+    if (st) return stream_records(a, *st, d_rec, d_index, n_rec, cap, n_out, w.stats.scan_ms);
     return finish(w.stats.scan_ms);
   }
   // prefilter engine over the whole span, each match bounded by its document (PrefilterLaunch::doc_offsets)
@@ -1998,7 +2086,85 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     w.stats.launches += 1;
   }
   CK(cudaEventRecord(w.ev3, w.stream));
+  if (st) return stream_records(a, *st, d_rec, d_index, r.n, cap, n_out, w.stats.order_ms);
   return finish(w.stats.order_ms);
+}
+
+// acg_streams_feed / acg_streams_feed_devout (include/acb200.h).  dev_out: `out` and `match_offsets` are device
+// arrays, else `out` is a host array.  The chunk offsets are checked (on the device when they are there) and D's
+// length fetched in one round trip; D is gathered, searched by batch_impl and its records finished by
+// stream_records.  Staging and gather time go to h2d_ms.
+int streams_feed_impl(acg_streams* set, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
+                      const uint64_t* chunk_offsets, bool offsets_on_device, uint64_t n_streams, uint64_t* out,
+                      uint64_t cap, uint64_t* match_offsets, bool dev_out, uint64_t* n_out) {
+  if (!set || !chunk_offsets || !n_out || n_streams != set->n || (dev_out && !match_offsets) || (!out && cap))
+    return ACG_E_INVALID_ARG;
+  *n_out = 0;
+  const uint64_t n = set->n, n1 = n + 1;
+  if (offsets_on_device) {
+    if (reinterpret_cast<uintptr_t>(chunk_offsets) & 7) return ACG_E_INVALID_ARG;
+  } else {
+    for (uint64_t i = 0; i < n; ++i)
+      if (chunk_offsets[i + 1] < chunk_offsets[i]) return ACG_E_INVALID_SPAN;
+    if (chunk_offsets[n] > hay_len) return ACG_E_INVALID_SPAN;
+  }
+  const acg_dfa* a = set->a;
+  DeviceGuard guard(a->device);
+  WsLease lease(a);
+  if (lease.rc) return lease.rc;
+  Workspace& w = cur_ws();
+  int rc = w.d_soffs.reserve(2 * n1);
+  if (rc) return rc;
+  acb::StreamLaunch p{};
+  p.n = n;
+  p.back = set->back;
+  p.overlapping = set->overlapping;
+  p.pos = set->d_state;
+  p.cursor = set->d_state + n;
+  p.tail = set->d_tail;
+  p.doc_offsets = reinterpret_cast<unsigned long long*>(w.d_soffs.p);
+  CK(cudaEventRecord(w.ev0, w.stream));
+  if (offsets_on_device) {
+    p.chunk_offsets = chunk_offsets;
+    CK(cudaMemsetAsync(w.d_counter, 0, 8, w.stream));
+    CK(acb::launch_check_offsets(chunk_offsets, n, hay_len, w.d_counter, w.stream));
+    CK(cudaMemcpyAsync(w.h_counter, w.d_counter, 24, cudaMemcpyDeviceToHost, w.stream));
+    w.stats.launches += 1;
+  } else {
+    p.chunk_offsets = w.d_soffs + n1;
+    CK(cudaMemcpyAsync(w.d_soffs + n1, chunk_offsets, n1 * 8, cudaMemcpyHostToDevice, w.stream));
+  }
+  CK(acb::launch_stream_docs(p, w.stream));
+  if ((rc = cub_call(w, [&](void* tmp, size_t& tb) {
+         return acb::inclusive_sum_u64(tmp, tb, p.doc_offsets + 1, p.doc_offsets + 1, n, w.stream);
+       })))
+    return rc;
+  CK(cudaMemcpyAsync(w.h_counter + 3, p.doc_offsets + n, 8, cudaMemcpyDeviceToHost, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  w.stats.launches += 2;
+  uint64_t chunks_lo = offsets_on_device ? w.h_counter[1] : chunk_offsets[0];
+  uint64_t chunks_hi = offsets_on_device ? w.h_counter[2] : chunk_offsets[n];
+  if (offsets_on_device && w.h_counter[0]) return ACG_E_INVALID_SPAN;
+  p.docs_len = w.h_counter[3];
+  // host chunks: staged in the workspace, read from there with their absolute offsets
+  Placement pl;
+  if ((rc = place_input(a, hay, hay_on_device, hay_len, chunks_lo, chunks_hi, false, &pl))) return rc;
+  p.chunks = pl.base;
+  if ((rc = w.d_sdocs.reserve(((p.docs_len + 64 + (1ull << 20)) >> 20) << 20))) return rc;
+  p.docs = w.d_sdocs;
+  if (p.docs_len) {
+    CK(acb::launch_stream_gather(p, w.stream));
+    w.stats.launches += 1;
+  }
+  CK(cudaEventRecord(w.ev1, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+  w.stats.h2d_ms = ms;
+  BatchStreams st{p, p.docs_len, out, dev_out ? match_offsets : nullptr};
+  return batch_impl(a, set->overlapping ? kBatchOverlapping : kBatchFindIter, p.docs, true, p.docs_len,
+                    w.d_soffs, n, 0, reinterpret_cast<acg_match*>(out), cap, n_out, nullptr, 0, nullptr, nullptr,
+                    nullptr, nullptr, &st);
 }
 
 }  // namespace
@@ -2448,6 +2614,85 @@ int acg_replace_all_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t h
   const BatchReplace rp{rep_bytes, rep_offsets, n_reps, d_out, d_out_offsets};
   return batch_impl(a, kBatchFindIter, static_cast<const uint8_t*>(d_hay), true, hay_len, doc_offsets, n_docs, 0,
                     nullptr, cap, out_len, nullptr, 0, &dv, nullptr, nullptr, &rp);
+}
+
+int acg_streams_create(const acg_dfa* a, uint64_t n_streams, int overlapping, acg_streams** out) {
+  if (!a || !out || n_streams == 0 || n_streams >= (1ull << 32)) return ACG_E_INVALID_ARG;
+  *out = nullptr;
+  // StreamChunkIter::new, src/automaton.rs:1087-1103, and try_find_overlapping_iter, :397-423
+  if (a->h.match_kind != ACG_STANDARD) return overlapping ? ACG_E_UNSUPPORTED_OVERLAPPING : ACG_E_UNSUPPORTED_STREAM;
+  if (a->has_empty) return ACG_E_UNSUPPORTED_EMPTY;
+  int rc = check_anchored(a->h.start_kind, 0);
+  if (rc || (rc = check_start(a->h, 0))) return rc;
+  if (!a->on_device) return ACG_E_NO_DEVICE;
+  acg_streams* s = new (std::nothrow) acg_streams();
+  if (!s) return ACG_E_NOMEM;
+  s->a = a;
+  s->n = n_streams;
+  s->back = a->h.max_pattern_len ? a->h.max_pattern_len - 1 : 0;
+  s->overlapping = overlapping != 0;
+  DeviceGuard guard(a->device);
+  cudaError_t e = cudaMalloc(&s->d_state, n_streams * 16);
+  if (e != cudaSuccess) s->d_state = nullptr;
+  if (e == cudaSuccess && (e = cudaMalloc(&s->d_tail, std::max<uint64_t>(n_streams * s->back, 16))) != cudaSuccess)
+    s->d_tail = nullptr;
+  if (e == cudaSuccess) e = cudaMemset(s->d_state, 0, n_streams * 16);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    acg_streams_free(s);
+    return e == cudaErrorMemoryAllocation ? ACG_E_NOMEM : ACG_E_CUDA;
+  }
+  *out = s;
+  return ACG_OK;
+}
+
+void acg_streams_free(acg_streams* s) {
+  if (!s) return;
+  {
+    DeviceGuard guard(s->a->device);
+    cudaFree(s->d_state);
+    cudaFree(s->d_tail);
+  }
+  delete s;
+}
+
+int acg_streams_reset(acg_streams* s, const uint64_t* ids, uint64_t n_ids) {
+  if (!s) return ACG_E_INVALID_ARG;
+  if (ids)
+    for (uint64_t i = 0; i < n_ids; ++i)
+      if (ids[i] >= s->n) return ACG_E_INVALID_ARG;
+  DeviceGuard guard(s->a->device);
+  if (!ids) {
+    CK(cudaMemset(s->d_state, 0, s->n * 16));
+    return ACG_OK;
+  }
+  std::vector<uint64_t> st(2 * s->n);
+  CK(cudaMemcpy(st.data(), s->d_state, s->n * 16, cudaMemcpyDeviceToHost));
+  for (uint64_t i = 0; i < n_ids; ++i) st[ids[i]] = st[s->n + ids[i]] = 0;
+  CK(cudaMemcpy(s->d_state, st.data(), s->n * 16, cudaMemcpyHostToDevice));
+  return ACG_OK;
+}
+
+int acg_streams_positions(const acg_streams* s, uint64_t* pos) {
+  if (!s || !pos) return ACG_E_INVALID_ARG;
+  DeviceGuard guard(s->a->device);
+  CK(cudaMemcpy(pos, s->d_state, s->n * 8, cudaMemcpyDeviceToHost));
+  return ACG_OK;
+}
+
+int acg_streams_feed(acg_streams* s, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                     const uint64_t* chunk_offsets, uint64_t n_streams, acg_doc_match* out, uint64_t cap,
+                     uint64_t* n_out) {
+  return streams_feed_impl(s, hay, hay_on_device != 0, hay_len, chunk_offsets, false, n_streams,
+                           reinterpret_cast<uint64_t*>(out), cap, nullptr, false, n_out);
+}
+
+int acg_streams_feed_devout(acg_streams* s, const void* d_hay, uint64_t hay_len, const uint64_t* chunk_offsets,
+                            int offsets_on_device, uint64_t n_streams, acg_doc_match* d_out, uint64_t cap,
+                            uint64_t* d_match_offsets, uint64_t* n_out) {
+  return streams_feed_impl(s, static_cast<const uint8_t*>(d_hay), true, hay_len, chunk_offsets,
+                           offsets_on_device != 0, n_streams, reinterpret_cast<uint64_t*>(d_out), cap,
+                           d_match_offsets, true, n_out);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

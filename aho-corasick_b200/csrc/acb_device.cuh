@@ -252,6 +252,43 @@ cudaError_t launch_replace_rows(const ReplaceLaunch& r, cudaStream_t s);
 uint64_t replace_splice_tiles(const uint8_t* out, uint64_t out_len);
 cudaError_t launch_replace_splice(const ReplaceLaunch& r, cudaStream_t s);
 
+// Stream sets (acg_streams_*): n streams over one automaton.  Stream s has received pos[s] bytes; cursor[s] is where
+// find_iter restarts (the end of the last match returned; always 0 in overlapping mode), and its tail is its bytes
+// [pos - L_s, pos), L_s = min(back, pos[s] - cursor[s]), stored at tail[s * back].  A feed runs:
+//   launch_stream_docs     doc_offsets[s + 1] = L_s + the length of chunk s, doc_offsets[0] = 0; an inclusive scan of
+//                          doc_offsets + 1 then makes them the CSR bounds of the combined documents D_s = tail_s | chunk_s
+//   launch_stream_gather   D into `docs`, 16-byte stores, one 4 KiB tile per CTA
+//   (the batch search of D: the records rec[m * 3], offsets relative to D_s, and their index rec_index[n + 1])
+//   launch_stream_keep     overlapping: keep[i] = 0 if record i ends inside its tail (a previous feed returned it), else
+//                          1; an inclusive scan of keep then numbers the kept records
+//   launch_stream_records  the kept records at out[j * 3], rebased to stream offsets (+ pos - L_s), and out_index
+//   launch_stream_state    pos, cursor and the new tail: D_s[t - (pos - L_s) ..) with t = max(pos' - back, cursor')
+// Nothing before launch_stream_state writes the state, so a feed that stops before it leaves every stream as it was.
+struct StreamLaunch {
+  uint64_t n;                       // streams
+  uint64_t back;                    // max_pattern_len - 1: the tail stride
+  int overlapping;
+  uint64_t* pos;                    // [n]
+  uint64_t* cursor;                 // [n]
+  uint8_t* tail;                    // [n * back]
+  const uint8_t* chunks;            // chunk s is chunks[chunk_offsets[s] .. chunk_offsets[s + 1])
+  const uint64_t* chunk_offsets;    // [n + 1]
+  unsigned long long* doc_offsets;  // [n + 1]
+  uint8_t* docs;                    // [docs_len], 16-byte aligned
+  uint64_t docs_len;
+  const uint64_t* rec;              // [m * 3] acg_doc_match records of D, document-major
+  const uint64_t* rec_index;        // [n + 1]
+  uint64_t m;
+  unsigned long long* keep;         // overlapping: [m]; nullptr: every record is kept
+  uint64_t* out;                    // [kept * 3]
+  uint64_t* out_index;              // [n + 1] or nullptr
+};
+cudaError_t launch_stream_docs(const StreamLaunch& p, cudaStream_t s);
+cudaError_t launch_stream_gather(const StreamLaunch& p, cudaStream_t s);  // docs_len > 0
+cudaError_t launch_stream_keep(const StreamLaunch& p, cudaStream_t s);    // m > 0
+cudaError_t launch_stream_records(const StreamLaunch& p, cudaStream_t s);
+cudaError_t launch_stream_state(const StreamLaunch& p, cudaStream_t s);
+
 // Offsets in device memory: result[0] = 1 if some offs[i] > offs[i + 1] or offs[n_docs] > hay_len (left as it
 // was otherwise: the caller clears it), result[1] = offs[0], result[2] = offs[n_docs].
 cudaError_t launch_check_offsets(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,

@@ -21,6 +21,11 @@
 //        replace_rows_kernel      the output offsets by document, the first match of every output tile,
 //        replace_tiles_kernel     and the output spliced tile by tile
 //        replace_splice_kernel
+//        stream_docs_kernel       a stream set's feed: the combined documents tail | chunk, gathered, the
+//        stream_gather_kernel     records that a previous feed has not returned, rebased to stream offsets,
+//        stream_keep_kernel       and every stream's new position, cursor and tail
+//        stream_records_kernel
+//        stream_state_kernel
 //        check_offsets_kernel     validation of document offsets in device memory
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
@@ -640,6 +645,132 @@ __global__ void __launch_bounds__(kSpliceThreads) replace_splice_kernel(ReplaceL
   }
 }
 
+// ---- stream sets (StreamLaunch) ----
+__device__ __forceinline__ uint64_t stream_tail_len(const StreamLaunch& p, uint64_t s) {
+  const uint64_t k = p.pos[s] - p.cursor[s];
+  return k < p.back ? k : p.back;
+}
+
+__global__ void stream_docs_kernel(StreamLaunch p) {
+  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s == 0) p.doc_offsets[0] = 0;
+  if (s >= p.n) return;
+  p.doc_offsets[s + 1] = stream_tail_len(p, s) + (p.chunk_offsets[s + 1] - p.chunk_offsets[s]);
+}
+
+// The last stream s in [lo, hi) with doc_offsets[s] <= o (lo - 1 if none): for o < docs_len the one whose D holds o.
+__device__ __forceinline__ int64_t stream_at(const StreamLaunch& p, int64_t lo, int64_t hi, uint64_t o) {
+  while (lo < hi) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    if (p.doc_offsets[mid] <= o) lo = mid + 1; else hi = mid;
+  }
+  return lo - 1;
+}
+
+// D in tiles of kSpliceTile bytes, one aligned 16-byte chunk per thread.  Two threads find the streams of the tile's
+// first and last byte, so each thread searches only among the tile's streams.  A chunk inside one stream's chunk or
+// tail bytes is one 16-byte copy; one that crosses a boundary is gathered byte by byte.
+__global__ void __launch_bounds__(kSpliceThreads) stream_gather_kernel(StreamLaunch p) {
+  __shared__ int64_t s_range[2];
+  const uint64_t tile0 = (uint64_t)blockIdx.x * kSpliceTile;
+  if (threadIdx.x < 2) {
+    const uint64_t last = (tile0 + kSpliceTile < p.docs_len ? tile0 + kSpliceTile : p.docs_len) - 1;
+    s_range[threadIdx.x] = stream_at(p, 0, (int64_t)p.n, threadIdx.x ? last : tile0);
+  }
+  __syncthreads();
+  const uint64_t o = tile0 + threadIdx.x * 16;
+  if (o >= p.docs_len) return;
+  const uint64_t n = p.docs_len - o < 16 ? p.docs_len - o : 16;
+  int64_t s = stream_at(p, s_range[0], s_range[1] + 1, o);
+  // the bytes of stream s: tail [d0, c0), chunk [c0, d1)
+  uint64_t d0, c0, d1;
+  const uint8_t *tail, *chunk;
+  auto enter = [&]() {
+    d0 = p.doc_offsets[s];
+    d1 = p.doc_offsets[s + 1];
+    c0 = d0 + stream_tail_len(p, (uint64_t)s);
+    tail = p.tail + (uint64_t)s * p.back;
+    chunk = p.chunks + p.chunk_offsets[s];
+  };
+  enter();
+  uint8_t* dst = p.docs + o;
+  if (n == 16 && o >= c0 && o + 16 <= d1) {
+    *reinterpret_cast<uint4*>(dst) = load16(chunk + (o - c0));
+    return;
+  }
+  if (n == 16 && o + 16 <= c0) {
+    *reinterpret_cast<uint4*>(dst) = load16(tail + (o - d0));
+    return;
+  }
+  uint64_t w0 = 0, w1 = 0;
+  for (uint64_t j = 0; j < n; ++j) {
+    const uint64_t q = o + j;
+    while (q >= d1) {
+      ++s;
+      enter();
+    }
+    const uint64_t b = q < c0 ? tail[q - d0] : chunk[q - c0];
+    if (j < 8) w0 |= b << (8 * j); else w1 |= b << (8 * (j - 8));
+  }
+  if (n == 16) {
+    *reinterpret_cast<uint4*>(dst) = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
+  } else {
+    for (uint64_t j = 0; j < n; ++j) dst[j] = (uint8_t)((j < 8 ? w0 >> (8 * j) : w1 >> (8 * (j - 8))) & 0xFF);
+  }
+}
+
+__global__ void stream_keep_kernel(StreamLaunch p) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.m) return;
+  const uint64_t* r = p.rec + i * 3;
+  p.keep[i] = r[2] > stream_tail_len(p, r[0] >> 32);
+}
+
+// Thread i < m: record i, if kept, at its place among the kept ones; thread i <= n: out_index[i], the kept records
+// before stream i's first one.
+__global__ void stream_records_kernel(StreamLaunch p) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < p.m) {
+    const uint64_t* r = p.rec + i * 3;
+    const bool kept = !p.keep || p.keep[i] != (i ? p.keep[i - 1] : 0ull);
+    if (kept) {
+      const uint64_t j = p.keep ? p.keep[i] - 1 : i, s = r[0] >> 32;
+      const uint64_t base = p.pos[s] - stream_tail_len(p, s);
+      p.out[j * 3 + 0] = r[0];
+      p.out[j * 3 + 1] = base + r[1];
+      p.out[j * 3 + 2] = base + r[2];
+    }
+  }
+  if (p.out_index && i <= p.n) {
+    const uint64_t first = p.rec_index[i];
+    p.out_index[i] = p.keep ? (first ? p.keep[first - 1] : 0) : first;
+  }
+}
+
+// One warp per stream: every lane reads the old state, then the new tail is copied and lane 0 stores pos and cursor.
+__global__ void stream_state_kernel(StreamLaunch p) {
+  const uint64_t s = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31;
+  if (s >= p.n) return;
+  const uint64_t d0 = p.doc_offsets[s];
+  const uint64_t base = p.pos[s] - stream_tail_len(p, s), pos = base + (p.doc_offsets[s + 1] - d0);
+  uint64_t cursor = p.cursor[s];
+  if (!p.overlapping) {
+    const uint64_t lo = p.rec_index[s], hi = p.rec_index[s + 1];
+    if (hi > lo) cursor = base + p.rec[(hi - 1) * 3 + 2];
+  }
+  uint64_t t = pos > p.back ? pos - p.back : 0;
+  if (cursor > t) t = cursor;
+  const uint8_t* src = p.docs + d0 + (t - base);
+  uint8_t* dst = p.tail + s * p.back;
+  for (uint64_t k = lane; k < pos - t; k += 32) dst[k] = src[k];
+  __syncwarp();
+  if (lane == 0) {
+    p.pos[s] = pos;
+    p.cursor[s] = cursor;
+  }
+}
+
 __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
                                      unsigned long long* result) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -813,6 +944,32 @@ cudaError_t launch_replace_splice(const ReplaceLaunch& r, cudaStream_t s) {
   const uint64_t mis = reinterpret_cast<uintptr_t>(r.out) & 15, n_tiles = replace_splice_tiles(r.out, r.out_len);
   ACB_LAUNCH(replace_tiles_kernel, (unsigned)((n_tiles + 1 + 255) / 256), 256, 0, s, r, n_tiles, mis);
   ACB_LAUNCH(replace_splice_kernel, (unsigned)n_tiles, kSpliceThreads, 0, s, r, mis);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_docs(const StreamLaunch& p, cudaStream_t s) {
+  ACB_LAUNCH(stream_docs_kernel, (unsigned)((p.n + 255) / 256), 256, 0, s, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_gather(const StreamLaunch& p, cudaStream_t s) {
+  ACB_LAUNCH(stream_gather_kernel, (unsigned)((p.docs_len + kSpliceTile - 1) / kSpliceTile), kSpliceThreads, 0, s, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_keep(const StreamLaunch& p, cudaStream_t s) {
+  ACB_LAUNCH(stream_keep_kernel, (unsigned)((p.m + 255) / 256), 256, 0, s, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_records(const StreamLaunch& p, cudaStream_t s) {
+  const uint64_t n = p.m > p.n + 1 ? p.m : p.n + 1;
+  ACB_LAUNCH(stream_records_kernel, (unsigned)((n + 255) / 256), 256, 0, s, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_state(const StreamLaunch& p, cudaStream_t s) {
+  ACB_LAUNCH(stream_state_kernel, (unsigned)((p.n * 32 + 255) / 256), 256, 0, s, p);
   return cudaGetLastError();
 }
 

@@ -334,6 +334,53 @@ int acg_replace_all_batch_devout(const acg_dfa* dfa, const void* d_hay, uint64_t
                                  const uint8_t* rep_bytes, const uint64_t* rep_offsets, uint64_t n_reps,
                                  uint8_t* d_out, uint64_t cap, uint64_t* d_out_offsets, uint64_t* out_len);
 
+/* ---- stream sets: many byte streams, each searched as its bytes arrive ----------------------
+ * A stream set holds n_streams streams over one automaton, in find_iter mode (overlapping == 0:
+ * the matches of try_find_iter, Standard semantics) or overlapping mode (the matches of
+ * try_find_overlapping_iter).  Let X_s be the bytes stream s has received since the set was
+ * created or the stream was last reset.  A feed takes one chunk per stream, in the batch form:
+ * chunk s is hay[chunk_offsets[s] .. chunk_offsets[s + 1]), empty chunks allowed.  A successful
+ * feed that takes X_s from n0 to n1 bytes returns, for every s, exactly the matches of the mode's
+ * iterator over all of X_s whose end lies in (n0, n1], as acg_doc_match records with doc = s and
+ * start / end absolute offsets into X_s, in ascending s and, within a stream, in the iterator's
+ * order.  So a stream's records over all its feeds, concatenated, are the iterator over X_s, and
+ * in find_iter mode also what try_stream_find_iter yields over X_s: a match that starts in one
+ * feed's bytes and ends in a later one's is returned once, by the later feed.
+ * Creation (the restrictions of StreamChunkIter::new and try_find_overlapping_iter):
+ * - a leftmost automaton gives ACG_E_UNSUPPORTED_STREAM (find_iter) or
+ *   ACG_E_UNSUPPORTED_OVERLAPPING (overlapping);
+ * - an automaton with the empty pattern gives ACG_E_UNSUPPORTED_EMPTY;
+ * - an automaton built with ACG_START_ANCHORED gives ACG_E_INVALID_INPUT_UNANCHORED;
+ * - n_streams == 0 or n_streams >= 2^32 gives ACG_E_INVALID_ARG;
+ * - ACG_E_NOMEM when the state does not fit: 16 bytes and max_pattern_len - 1 tail bytes per
+ *   stream, on the automaton's device.  The automaton must outlive the set.
+ * Feeds: hay_on_device != 0 (always for _devout): hay is a device pointer to byte 0.  Decreasing
+ * chunk offsets or offsets past hay_len give ACG_E_INVALID_SPAN (detected on the device when the
+ * offsets are there); n_streams other than the set's, a NULL n_out, a NULL out with cap > 0 or a
+ * NULL d_match_offsets give ACG_E_INVALID_ARG.  If *n_out > cap the call returns ACG_E_OVERFLOW
+ * with the required count in *n_out and writes nothing (two-call protocol): a retry with room
+ * returns what the first call would have.  Every error leaves every stream as it was, except
+ * ACG_E_CUDA, after which the set's state is undefined until acg_streams_reset(set, NULL, 0).
+ * _devout: d_out and d_match_offsets[n_streams + 1] (the CSR index of the records by stream, as in
+ * the batch _devout calls) are device pointers, chunk_offsets as doc_offsets there; n_out is a
+ * host pointer.  The engine is that of the batch calls, chosen per feed.
+ * One call at a time per set (feed, reset, positions): the caller serialises them.  Different sets,
+ * also on one automaton, may be fed from different threads at once.
+ * acg_streams_reset: ids (host memory, n_ids entries) restart from zero bytes; ids == NULL resets
+ * every stream.  An id >= n_streams gives ACG_E_INVALID_ARG and resets none.
+ * acg_streams_positions: pos[s] = the length of X_s, pos in host memory with n_streams entries. */
+typedef struct acg_streams acg_streams;
+int acg_streams_create(const acg_dfa* dfa, uint64_t n_streams, int overlapping, acg_streams** out);
+void acg_streams_free(acg_streams* set);
+int acg_streams_reset(acg_streams* set, const uint64_t* ids, uint64_t n_ids);
+int acg_streams_positions(const acg_streams* set, uint64_t* pos);
+int acg_streams_feed(acg_streams* set, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                     const uint64_t* chunk_offsets, uint64_t n_streams, acg_doc_match* out, uint64_t cap,
+                     uint64_t* n_out);
+int acg_streams_feed_devout(acg_streams* set, const void* d_hay, uint64_t hay_len, const uint64_t* chunk_offsets,
+                            int offsets_on_device, uint64_t n_streams, acg_doc_match* d_out, uint64_t cap,
+                            uint64_t* d_match_offsets, uint64_t* n_out);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

@@ -546,6 +546,87 @@ class AhoCorasick {
   mutable uint64_t cap_hint_ = 4096;
 };
 
+// A stream set (acg_streams_*, include/acb200.h): n streams searched on the device as their bytes arrive.  feed()
+// takes one chunk per stream -- CSR `offsets` [n + 1] into `chunks` -- and returns, per stream, the matches of the
+// mode's iterator (find_iter, or find_overlapping_iter when `overlapping`) over all the stream's bytes that end in
+// this chunk, with offsets into the whole stream.  The automaton must outlive the set; one call at a time per set.
+class Streams {
+ public:
+  Streams(const AhoCorasick& ac, uint64_t n_streams, bool overlapping = false) {
+    Result<int> r;
+    r.error = acg_streams_create(ac.raw(), n_streams, overlapping, &h_);
+    r.unwrap();
+    n_ = n_streams;
+  }
+  Streams(Streams&& o) noexcept : h_(o.h_), n_(o.n_), cap_hint_(o.cap_hint_) { o.h_ = nullptr; }
+  Streams& operator=(Streams&& o) noexcept {
+    if (this != &o) { close(); h_ = o.h_; n_ = o.n_; cap_hint_ = o.cap_hint_; o.h_ = nullptr; }
+    return *this;
+  }
+  Streams(const Streams&) = delete;
+  Streams& operator=(const Streams&) = delete;
+  ~Streams() { close(); }
+
+  uint64_t n_streams() const { return n_; }
+
+  using PerStream = std::vector<std::vector<Match>>;
+  Result<PerStream> try_feed(std::string_view chunks, const std::vector<uint64_t>& offsets) {
+    Result<PerStream> r;
+    std::vector<acg_doc_match> buf(std::max<uint64_t>(cap_hint_, 64));
+    uint64_t n = 0;
+    for (;;) {
+      const uint64_t n_chunks = offsets.empty() ? 0 : offsets.size() - 1;
+      const int rc = acg_streams_feed(h_, reinterpret_cast<const uint8_t*>(chunks.data()), 0, chunks.size(),
+                                      offsets.empty() ? nullptr : offsets.data(), n_chunks, buf.data(), buf.size(), &n);
+      if (rc == ACG_E_OVERFLOW) {  // nothing was fed: retry with room for n
+        cap_hint_ = n + n / 8 + 64;
+        buf.resize(cap_hint_);
+        continue;
+      }
+      r.error = rc;
+      break;
+    }
+    if (r.error == 0) {
+      r.value.resize(n_);
+      for (uint64_t i = 0; i < n; ++i) r.value[buf[i].doc].emplace_back(buf[i].pid, buf[i].start, buf[i].end);
+    }
+    return r;
+  }
+  PerStream feed(std::string_view chunks, const std::vector<uint64_t>& offsets) {
+    return std::move(try_feed(chunks, offsets).unwrap());
+  }
+  // Restart the given streams from zero bytes; reset() restarts every stream.
+  void reset(const std::vector<uint64_t>& ids) {
+    if (ids.empty()) return;
+    Result<int> r;
+    r.error = acg_streams_reset(h_, ids.data(), ids.size());
+    r.unwrap();
+  }
+  void reset() {
+    Result<int> r;
+    r.error = acg_streams_reset(h_, nullptr, 0);
+    r.unwrap();
+  }
+  // The bytes every stream has received.
+  std::vector<uint64_t> positions() const {
+    std::vector<uint64_t> pos(n_);
+    Result<int> r;
+    r.error = acg_streams_positions(h_, pos.data());
+    r.unwrap();
+    return pos;
+  }
+  acg_streams* raw() const { return h_; }
+
+ private:
+  void close() {
+    if (h_) acg_streams_free(h_);
+    h_ = nullptr;
+  }
+  acg_streams* h_ = nullptr;
+  uint64_t n_ = 0;
+  uint64_t cap_hint_ = 4096;
+};
+
 template <class Patterns>
 AhoCorasick AhoCorasickBuilder::build(const Patterns& patterns) const {
   std::vector<const uint8_t*> ptrs;

@@ -1,0 +1,204 @@
+#!/usr/bin/env python3
+"""Stream sets (acg_streams_feed_devout through Streams.feed_torch) on the two shapes either side of the chunk size.
+
+    python tools/bench_streams.py [--workload a|b|both] [--rounds-warmup 1] [--decode-feeds 1000]
+
+(a) cfg 2's 4 GiB haystack cut into its ~1.8 M documents (tools/bench_docs.py's seeds), dealt in order to 65 536
+    streams and fed in 16 rounds cut at document boundaries, overlapping mode, device output.  Every round's
+    chunks are gathered into one CUDA buffer (with CUDA int64 offsets) before the timed region.  Reported: the
+    host-clock time of each feed (the call ends in a device synchronise) and their total, against one
+    find_overlapping_iter_batch_torch over the same 65 536 streams' bytes in the same session (the result is
+    checked equal to the feeds' records); and, from torch.profiler over two more rounds, stream_gather_kernel's
+    bytes per second against a device-to-device copy of the same bytes timed with CUDA events.
+(b) cfg 4 (50 patterns), 4 096 streams, 4-byte chunks from CUDA tensors, find_iter mode, device output, as a
+    decode step.  Reported: the wall time per feed, the device time per feed (the sum of the kernels' durations
+    in a torch.profiler run of its own), the library's launch count per feed, and the share of the wall time
+    that no kernel covers (host round trips, launch gaps and Python).
+
+Prints one JSON line per workload with the card's name and power limit."""
+import argparse
+import json
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+ROOT = Path(__file__).resolve().parents[1]
+sys.path.insert(0, str(ROOT))
+sys.dont_write_bytecode = True
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                       text=True).stdout.strip().splitlines()
+    name, power = (q[0].split(", ") + ["?"])[:2] if q else ("?", "?")
+    return name, power
+
+
+def kernel_ms(prof, names=None):
+    """Sum of the CUDA kernels' device time (ms) in a torch.profiler run, optionally only those whose name holds one
+    of `names`."""
+    total = 0.0
+    for e in prof.events():
+        if e.device_type.name != "CUDA":
+            continue
+        if names and not any(n in e.name for n in names):
+            continue
+        total += e.device_time_total / 1000.0  # us
+    return total
+
+
+def gather_round(d_hay, lo, hi):
+    import torch
+    lens = hi - lo
+    offs = np.r_[0, np.cumsum(lens)].astype(np.int64)
+    total = int(offs[-1])
+    shift = torch.repeat_interleave(torch.from_numpy(lo - offs[:-1]).cuda(), torch.from_numpy(lens).cuda(),
+                                    output_size=total)
+    values = d_hay[torch.arange(total, device="cuda") + shift]
+    return values, torch.from_numpy(offs).cuda()
+
+
+def workload_a(args, ab, W):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    n = 4 << 30
+    pats = W.config_patterns("cfg2")
+    ac = ab.AhoCorasick.builder().kind(ab.AhoCorasickKind.DFA).build(pats)
+    d_hay = torch.empty(n, dtype=torch.uint8, device="cuda")
+    W.torch_fill_config("cfg2", d_hay, pats)
+    offs = W.doc_offsets(n, 0xD0C5)
+    n_docs, n_streams, rounds = offs.size - 1, 65536, 16
+    first = (np.arange(n_streams + 1) * n_docs) // n_streams
+    bounds = offs[first].astype(np.int64)
+    cuts = np.stack([offs[first[:-1] + ((first[1:] - first[:-1]) * r) // rounds] for r in range(rounds)]
+                    + [bounds[1:]]).astype(np.int64)
+    feeds = [gather_round(d_hay, cuts[r], cuts[r + 1]) for r in range(rounds)]
+    d_bounds = torch.from_numpy(bounds).cuda()
+    ac.find_overlapping_iter_batch_torch((d_hay, d_bounds))  # warm-up: capacities and modules
+    for _ in range(args.rounds_warmup):
+        with ac.streams(n_streams, True) as st:
+            for r in range(2):
+                st.feed_torch(feeds[r])
+    torch.cuda.synchronize()
+    times, parts = [], []
+    with ac.streams(n_streams, True) as st:
+        for r in range(rounds):
+            t0 = time.perf_counter()
+            got = st.feed_torch(feeds[r])
+            times.append((time.perf_counter() - t0) * 1e3)
+            parts.append(got.records.clone())
+    t0 = time.perf_counter()
+    want = ac.find_overlapping_iter_batch_torch((d_hay, d_bounds))
+    batch_ms = (time.perf_counter() - t0) * 1e3
+    batch_stats = ac.last_stats()
+    rec = torch.cat(parts)
+    rec = rec[torch.sort(rec[:, 0] >> 32, stable=True).indices]
+    same = bool(rec.shape == want.records.shape and torch.equal(rec, want.records))
+    # gather rate: the kernel's time over two rounds from the profiler, against a D2D copy of the same bytes
+    with ac.streams(n_streams, True) as st:
+        st.feed_torch(feeds[0])
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            st.feed_torch(feeds[1])
+            st.feed_torch(feeds[2])
+            torch.cuda.synchronize()
+        pos = st.positions()
+    gather_ms = kernel_ms(prof, ["stream_gather_kernel"])
+    back = ac.max_pattern_len() - 1
+    # bytes the gather wrote: every chunk plus every tail (at most `back` bytes per stream and feed)
+    chunk_bytes = int(feeds[1][0].numel() + feeds[2][0].numel())
+    tail_bound = 2 * n_streams * back
+    src = feeds[1][0]
+    dst = torch.empty_like(src)
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    dst.copy_(src)
+    ev0.record()
+    for _ in range(10):
+        dst.copy_(src)
+    ev1.record()
+    torch.cuda.synchronize()
+    d2d_ms = ev0.elapsed_time(ev1) / 10
+    name, power = card()
+    return {
+        "workload": "a: cfg2 4 GiB, 65536 streams x 16 rounds, overlapping, device output",
+        "gpu": name, "power_limit": power,
+        "feed_ms": [round(t, 3) for t in times], "feeds_total_ms": round(sum(times), 3),
+        "batch_call_ms": round(batch_ms, 3), "batch_scan_order_ms": round(batch_stats["scan_ms"] +
+                                                                          batch_stats["order_ms"], 3),
+        "records": int(rec.shape[0]), "equal_to_batch": same,
+        "gather_kernel_ms_2_feeds": round(gather_ms, 3), "gather_chunk_bytes": chunk_bytes,
+        "gather_tail_bytes_at_most": tail_bound,
+        "gather_GBps_chunk_bytes": round(chunk_bytes / gather_ms / 1e6, 1) if gather_ms else None,
+        "d2d_copy_ms_one_feed": round(d2d_ms, 3), "d2d_GBps_bytes_copied": round(src.numel() / d2d_ms / 1e6, 1),
+        "positions_checked": bool(pos.sum() == cuts[3].sum() - cuts[0].sum()),
+    }
+
+
+def workload_b(args, ab, W):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    n_streams, k = 4096, 4
+    pats = W.config_patterns("cfg4")
+    ac = ab.AhoCorasick.builder().kind(ab.AhoCorasickKind.DFA).build(pats)
+    feeds_n = args.decode_feeds
+    d_hay = torch.empty(n_streams * k * (feeds_n + 20), dtype=torch.uint8, device="cuda")
+    W.torch_fill_config("cfg4", d_hay, pats)
+    # feed i's chunk of stream s is 4 bytes of the stream's own range: stream s is d_hay[s * L, (s + 1) * L)
+    L = k * (feeds_n + 20)
+    base = torch.arange(n_streams, device="cuda") * L
+    offs = torch.arange(n_streams + 1, device="cuda", dtype=torch.int64) * k
+    lane = torch.arange(k, device="cuda")
+
+    def chunk(i):
+        return d_hay[(base[:, None] + i * k + lane[None, :]).reshape(-1)]
+
+    chunks = [chunk(i) for i in range(feeds_n + 20)]
+    torch.cuda.synchronize()
+    with ac.streams(n_streams) as st:
+        for i in range(20):
+            st.feed_torch((chunks[i], offs))
+        torch.cuda.synchronize()
+        times, launches, n_rec = [], [], 0
+        for i in range(20, 20 + feeds_n):
+            t0 = time.perf_counter()
+            got = st.feed_torch((chunks[i], offs))
+            times.append((time.perf_counter() - t0) * 1e3)
+            launches.append(ac.last_stats()["launches"])
+            n_rec += int(got.records.shape[0])
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            for i in range(20, 120):
+                st.feed_torch((chunks[i], offs))
+            torch.cuda.synchronize()
+    dev_ms = kernel_ms(prof) / 100
+    wall = float(np.median(times))
+    name, power = card()
+    return {
+        "workload": "b: cfg4, 4096 streams, 4-byte chunks from CUDA tensors, find_iter, device output",
+        "gpu": name, "power_limit": power, "feeds": feeds_n,
+        "wall_ms_per_feed_median": round(wall, 4), "wall_ms_per_feed_p90": round(float(np.percentile(times, 90)), 4),
+        "device_kernel_ms_per_feed": round(dev_ms, 4), "launches_per_feed": int(np.median(launches)),
+        "share_of_wall_outside_kernels": round(1 - dev_ms / wall, 3), "records": n_rec,
+    }
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="both", choices=["a", "b", "both"])
+    ap.add_argument("--rounds-warmup", type=int, default=1)
+    ap.add_argument("--decode-feeds", type=int, default=1000)
+    args = ap.parse_args()
+    import torch
+    assert torch.cuda.is_available(), "bench_streams.py needs a CUDA device"
+    import aho_corasick_b200 as ab
+    from aho_corasick_b200 import workload as W
+    if args.workload in ("a", "both"):
+        print(json.dumps(workload_a(args, ab, W)), flush=True)
+        torch.cuda.empty_cache()
+    if args.workload in ("b", "both"):
+        print(json.dumps(workload_b(args, ab, W)), flush=True)
+
+
+if __name__ == "__main__":
+    main()
