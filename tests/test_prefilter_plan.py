@@ -21,6 +21,9 @@ sys.path.insert(0, str(ROOT))
 import aho_corasick_b200 as ab  # noqa: E402
 from aho_corasick_b200 import workload as W  # noqa: E402
 
+sys.path.insert(0, str(ROOT / "tests"))
+import byte_families as F  # noqa: E402
+
 M32 = 0xFFFFFFFF
 
 
@@ -125,11 +128,20 @@ def le32(b4):
     return int.from_bytes(bytes(b4) + b"\0" * (4 - len(b4)), "little")
 
 
-def case_variants(rng, b, n):
+def case_variants(rng, b, n, partners=False):
+    """Spellings of b that match it under ascii_case_insensitive (letters flipped at random); with
+    `partners`, (spelling, is_match) pairs that add b with one non-letter swapped for its fold partner
+    (x ^ 0x20: the twelve punctuation / DEL bytes and every high byte), which must not match."""
     out = {bytes(b)}
     for _ in range(n):
         out.add(bytes((c ^ 0x20) if (chr(c).isalpha() and c < 128 and rng.random() < 0.5) else c for c in b))
-    return out
+    if not partners:
+        return out
+    pairs = {(v, True) for v in out}
+    for i, c in enumerate(b):
+        if not (chr(c).isalpha() and c < 128):
+            pairs.add((bytes(b[:i]) + bytes([c ^ 0x20]) + bytes(b[i + 1:]), False))
+    return pairs
 
 
 def set_experiment(ac, flags):
@@ -155,9 +167,26 @@ def check(pats, experiment=0, **knobs):
     rng = random.Random(len(pats))
     stride2 = int(t["stride2"])
     for pat in pats:
-        for v in (case_variants(rng, pat, 3) if ci else {bytes(pat)}):
-            # the text "v + tail" at an even and at an odd offset: the probes that must fire
+        for v, spelling in (case_variants(rng, pat, 3, partners=True) if ci else {(bytes(pat), True)}):
+            # the text "v + tail" at an even and at an odd offset: the probes that must fire.  A fold
+            # partner spelling is merged with the pattern by the fold; without one it may miss.
             w0 = le32(v[:4])
+            if not spelling:
+                if p.fold == (0x20202020 & p.kmask) and not p.brute:
+                    if p.stride == 2:
+                        assert first_stage_hit(p, w0)
+                        if len(v) > 4:
+                            assert first_stage_hit(p, le32(v[1:5]))
+                    else:
+                        assert first_stage_hit(p, w0)
+                    assert second_stage_hit(p, w0)
+                # the anchor map is keyed by raw bytes: a state only if the spelling is itself a pattern start
+                sid = anchor_lookup(p, w0 & p.kmask)
+                if sid is not None:
+                    key = v[:p.k]
+                    on_path = walk(t, key) != 0 and p.depth16[walk(t, key) >> stride2] == p.k
+                    assert sid == (walk(t, key) if on_path else 0), (pat, v)
+                continue
             if not p.brute:
                 if p.stride == 2:
                     assert p.k == 4
@@ -281,3 +310,45 @@ def test_27_bit_keys_cut_the_first_stage_pass_rate():
     # the genuine 3-byte prefix hits (10 000 fingerprints in 95^3) all but disappear; what remains are the
     # Bloom false positives of a bitmap that also carries the second stage's two bits per 4-gram
     assert again == k27 and k27 < base * 0.97
+
+
+# the families of the device rows in test_gpu_byte_content.py (all but the 270 000-pattern set, whose
+# per-pattern restated probes take minutes in Python): (patterns, knobs, experiment flags, expected plan)
+BYTE_FAMILIES = {
+    "high-narrow": (lambda: F.high(5000, 0xB1), {}, 0, dict(stride=2, wide=0, dense=0, fold=0)),
+    "high-wide": (lambda: F.high(50, 0xB2), {}, 0, dict(stride=2, wide=1, fold=0)),
+    "high-dense": (lambda: F.high(20000, 0xB3), {}, 0, dict(stride=1, dense=1, fold=0)),
+    "high-k3": (lambda: F.high(300, 0xB4, 3, 12), {}, 0, dict(stride=1, dense=0, k=3)),
+    "high-k2": (lambda: F.high(300, 0xB5, 2, 12), {}, 0, dict(stride=1, dense=0, k=2)),
+    "high-k1": (lambda: F.high(300, 0xB6, 1, 12), {}, 0, dict(brute=1, k=1, fold=0x20)),
+    "full-narrow": (lambda: F.full(5000, 0xF1), {}, 0, dict(stride=2, wide=0, dense=0)),
+    "full-wide": (lambda: F.full(50, 0xF2), {}, 0, dict(stride=2, wide=1)),
+    "full-dense": (lambda: F.full(20000, 0xF3), {}, 0, dict(stride=1, dense=1)),
+    "full-k3": (lambda: F.full(300, 0xF4, 3, 12), {}, 0, dict(stride=1, dense=0, k=3)),
+    "fold-ci-narrow": (lambda: F.fold_mix(5000, 0xC1), dict(ascii_case_insensitive=True), 0,
+                       dict(stride=2, wide=0, dense=0, fold=0x20202020)),
+    "fold-ci-dense": (lambda: F.fold_mix(20000, 0xC2), dict(ascii_case_insensitive=True), 0,
+                      dict(stride=1, dense=1, fold=0x20202020)),
+    "fold-ci-leftmost": (lambda: F.fold_mix(5000, 0xC1),
+                         dict(ascii_case_insensitive=True, match_kind=ab.MatchKind.LeftmostLongest), 0,
+                         dict(stride=2, wide=0, fold=0x20202020)),
+    "spellings": (lambda: F.spellings(1700, 0x5E), {}, 0, dict(stride=1, dense=0, k=4, fold=0x20202020)),
+    "keys4-key27": (lambda: F.keys4(2000, 0x4B), {}, 0, dict(stride=2, key_shift=5)),
+    "keys4-key24": (lambda: F.keys4(2000, 0x4B), {}, 8, dict(stride=2, key_shift=8)),
+    "needles3": (lambda: F.needles(F.NEEDLES3, 300, 0x3D), {}, 0, dict(brute=1, bs_n=3)),
+    "needles4": (lambda: F.needles(F.NEEDLES4, 300, 0x4D), {}, 0, dict(brute=1, bs_n=0)),
+    "nobc-narrow": (lambda: F.high(5000, 0xB1), dict(byte_classes=False), 0, dict(stride=2, wide=0, dense=0)),
+    "nobc-dense": (lambda: F.high(20000, 0xB3), dict(byte_classes=False), 0, dict(stride=1, dense=1)),
+}
+
+
+@pytest.mark.parametrize("family", list(BYTE_FAMILIES))
+def test_plan_on_byte_content_families(family):
+    """High bytes, NUL / DEL, fold-pair non-letters, case spellings, 4-byte keys and needle sets: no false
+    negatives at either stride-2 alignment; under case insensitivity the fold-partner spellings of
+    non-letters and high bytes reach the first stage and get no anchor-map state."""
+    make, knobs, experiment, want = BYTE_FAMILIES[family]
+    p = check(make(), experiment=experiment, **knobs)
+    assert p.supported
+    got = {k: getattr(p, k) for k in want}
+    assert got == want, (family, got)
