@@ -176,6 +176,12 @@ def _declare(lib):
     lib.acg_streams_positions.argtypes = [_vp, _vp]
     lib.acg_streams_feed.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _vp, _u64, C.POINTER(_u64)]
     lib.acg_streams_feed_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _vp, _u64, _vp, C.POINTER(_u64)]
+    lib.acg_streams_create_replace.argtypes = [_vp, _u64, _vp, _vp, _u64, C.POINTER(_vp)]
+    lib.acg_streams_replace_feed.argtypes = [_vp, _vp, _i, _u64, _vp, _u64, _vp, _u64, _vp, C.POINTER(_u64)]
+    lib.acg_streams_replace_feed_devout.argtypes = [_vp, _vp, _u64, _vp, _i, _u64, _vp, _u64, _vp,
+                                                    C.POINTER(_u64)]
+    lib.acg_streams_flush.argtypes = [_vp, _vp, _u64, _vp, _u64, _vp, C.POINTER(_u64)]
+    lib.acg_streams_held.argtypes = [_vp, _vp]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -1189,6 +1195,13 @@ class AhoCorasick:
         feed returns the matches that end in the bytes it brought, with offsets into the whole stream."""
         return Streams(self, n_streams, overlapping)
 
+    def replace_streams(self, n_streams, replace_with):
+        """A set of n_streams byte streams whose text is replaced on the device as their bytes arrive
+        (acg_streams_create_replace): each feed returns, per stream, the text that can no longer change, with every
+        find_iter match replaced by replace_with[pattern] (the forms replace_all_batch takes).  A stream's outputs,
+        followed by its flush, are replace_all_bytes of everything it received, as stream_replace_all writes it."""
+        return ReplaceStreams(self, n_streams, replace_with)
+
     def try_stream_replace_all_with(self, rdr, wtr, replace_with, chunk_bytes=64 << 20):
         """`try_stream_replace_all_with`, src/ahocorasick.rs:1807 -> src/automaton.rs:601-636:
         `replace_with(match, matched bytes, wtr)` writes the replacement; text between matches is
@@ -1250,24 +1263,8 @@ class AhoCorasick:
         return cnt.value, fnv.value, ms.value
 
 
-class Streams:
-    """A stream set (include/acb200.h, acg_streams_*): n_streams streams over one automaton, in find_iter mode
-    (try_find_iter, Standard semantics) or overlapping mode (try_find_overlapping_iter).  A feed takes one chunk per
-    stream -- in any form the batch calls take -- and returns, per stream, the matches of the mode's iterator over
-    everything the stream has received whose end lies in this feed's bytes, offsets absolute within the stream.  A
-    stream's matches over all its feeds, concatenated, are the iterator over its concatenated chunks.  One call at a
-    time per set.  Create it with AhoCorasick.streams(); the automaton is kept alive by the set."""
-
-    def __init__(self, ac, n_streams, overlapping=False):
-        self._ac = ac
-        self._h = None
-        h = _vp()
-        rc = _lib.acg_streams_create(ac._h, int(n_streams), int(bool(overlapping)), C.byref(h))
-        if rc:
-            ac._raise(rc)
-        self._h = h
-        self.n_streams = int(n_streams)
-        self.overlapping = bool(overlapping)
+class _StreamSet:
+    """What every stream set (Streams, ReplaceStreams) has: its handle, its life cycle, reset and positions."""
 
     def close(self):
         if self._h and _lib is not None:
@@ -1291,6 +1288,56 @@ class Streams:
             raise ValueError("the stream set is closed")
         if n_chunks != self.n_streams:
             raise ValueError(f"a feed takes one chunk per stream: {n_chunks} chunks for {self.n_streams} streams")
+
+    @staticmethod
+    def _ids(ids):
+        """(keepalive uint64 array or None, its address or None, its length) of stream ids (None: every stream)."""
+        if ids is None:
+            return None, None, 0
+        a = np.ascontiguousarray(np.asarray(ids, dtype=np.int64).reshape(-1))
+        if (a < 0).any():
+            raise ValueError("stream ids must be non-negative")
+        a = a.astype(np.uint64)
+        return a, a.ctypes.data if a.size else None, a.size
+
+    def reset(self, ids=None):
+        """Restart the given streams (all when ids is None) from zero bytes."""
+        self._check(self.n_streams)
+        a, ptr, n = self._ids(ids)
+        if a is not None and n == 0:
+            return
+        rc = _lib.acg_streams_reset(self._h, ptr, n)
+        if rc:
+            self._ac._raise(rc)
+
+    def positions(self):
+        """The bytes every stream has received: uint64 [n_streams]."""
+        self._check(self.n_streams)
+        pos = np.empty(self.n_streams, dtype=np.uint64)
+        rc = _lib.acg_streams_positions(self._h, pos.ctypes.data)
+        if rc:
+            self._ac._raise(rc)
+        return pos
+
+
+class Streams(_StreamSet):
+    """A stream set (include/acb200.h, acg_streams_*): n_streams streams over one automaton, in find_iter mode
+    (try_find_iter, Standard semantics) or overlapping mode (try_find_overlapping_iter).  A feed takes one chunk per
+    stream -- in any form the batch calls take -- and returns, per stream, the matches of the mode's iterator over
+    everything the stream has received whose end lies in this feed's bytes, offsets absolute within the stream.  A
+    stream's matches over all its feeds, concatenated, are the iterator over its concatenated chunks.  One call at a
+    time per set.  Create it with AhoCorasick.streams(); the automaton is kept alive by the set."""
+
+    def __init__(self, ac, n_streams, overlapping=False):
+        self._ac = ac
+        self._h = None
+        h = _vp()
+        rc = _lib.acg_streams_create(ac._h, int(n_streams), int(bool(overlapping)), C.byref(h))
+        if rc:
+            ac._raise(rc)
+        self._h = h
+        self.n_streams = int(n_streams)
+        self.overlapping = bool(overlapping)
 
     def feed_np(self, chunks):
         """One chunk per stream (a list of bytes / str, or (values, offsets) as the batch calls take): the new
@@ -1322,27 +1369,97 @@ class Streams:
                 match_offsets.data_ptr(), C.byref(cnt)))
         return BatchMatches(r, match_offsets, r[:, 0] & 0xFFFFFFFF, r[:, 0] >> 32, r[:, 1], r[:, 2])
 
-    def reset(self, ids=None):
-        """Restart the given streams (all when ids is None) from zero bytes."""
-        self._check(self.n_streams)
-        if ids is None:
-            rc = _lib.acg_streams_reset(self._h, None, 0)
-        else:
-            a = np.ascontiguousarray(np.asarray(ids, dtype=np.int64).reshape(-1))
-            if (a < 0).any():
-                raise ValueError("stream ids must be non-negative")
-            if a.size == 0:
-                return
-            a = a.astype(np.uint64)
-            rc = _lib.acg_streams_reset(self._h, a.ctypes.data, a.size)
-        if rc:
-            self._ac._raise(rc)
 
-    def positions(self):
-        """The bytes every stream has received: uint64 [n_streams]."""
+class ReplaceStreams(_StreamSet):
+    """A replace set (include/acb200.h, acg_streams_create_replace): n_streams streams over one automaton (Standard
+    semantics) whose text comes back with every find_iter match replaced by its pattern's replacement.  A feed takes
+    one chunk per stream -- in any form Streams.feed* takes -- and returns per stream the bytes between the last
+    feed's emit boundary and this one's: everything before the boundary is settled, the at most
+    max_pattern_len - 1 bytes after it (held()) may still become part of a match.  flush() returns the held bytes
+    of the given streams and restarts them.  A stream's outputs over its feeds, followed by its flush, are
+    replace_all_bytes of its bytes.  The output is bytes: a boundary may fall inside a multi-byte UTF-8 character.
+    One call at a time per set.  Create it with AhoCorasick.replace_streams()."""
+
+    def __init__(self, ac, n_streams, replace_with):
+        self._ac = ac
+        self._h = None
+        rkeep, rptr, roffs = ac._replacement_table(replace_with)
+        h = _vp()
+        rc = _lib.acg_streams_create_replace(ac._h, int(n_streams), rptr, roffs.ctypes.data, roffs.size - 1,
+                                             C.byref(h))
+        if rc:
+            ac._raise(rc)
+        self._h = h
+        self.n_streams = int(n_streams)
+
+    def feed_np(self, chunks):
+        """One chunk per stream (a list of bytes / str, or (values, offsets) as the batch calls take): the released
+        text as (values uint8, offsets uint64 [n_streams + 1]), stream s's at values[offsets[s]:offsets[s + 1]]."""
+        keep, ptr, n, on_dev, offs = _batch_input(chunks)
+        self._check(offs.size - 1)
+        out_offsets = np.empty(self.n_streams + 1, dtype=np.uint64)
+        values = self._ac._replace_until_it_fits(
+            int(offs[-1]) - int(offs[0]), lambda cap: np.empty(cap, dtype=np.uint8),
+            lambda out, cap, cnt: _lib.acg_streams_replace_feed(
+                self._h, ptr, on_dev, n, offs.ctypes.data, self.n_streams, out.ctypes.data, cap,
+                out_offsets.ctypes.data, cnt))
+        return values, out_offsets
+
+    def feed(self, chunks):
+        """One chunk per stream: one bytes object per stream."""
+        return self._split(*self.feed_np(chunks))
+
+    def feed_torch(self, chunks):
+        """(values, offsets) chunks with values a CUDA torch.uint8 tensor and offsets an int64 CUDA tensor on its
+        device or a host array: the released text as (values, CUDA uint8; offsets, CUDA int64 [n_streams + 1])."""
+        import torch
+        values, keep, optr, n_chunks, on_dev = _torch_batch(chunks)
+        self._check(n_chunks)
+        dev = values.device
+        span = values.numel() if on_dev else int(keep[-1]) - int(keep[0])
+        out_offsets = torch.empty(n_chunks + 1, dtype=torch.int64, device=dev)
+        out = self._ac._replace_until_it_fits(
+            span, lambda cap: torch.empty(cap, dtype=torch.uint8, device=dev),
+            lambda out, cap, cnt: _lib.acg_streams_replace_feed_devout(
+                self._h, values.data_ptr(), values.numel(), optr, on_dev, self.n_streams, out.data_ptr(), cap,
+                out_offsets.data_ptr(), cnt))
+        return out, out_offsets
+
+    def flush_np(self, ids=None):
+        """The held bytes of the given streams (all when ids is None), raw, as (values uint8, offsets uint64
+        [len(ids) + 1]); those streams then restart from zero bytes."""
         self._check(self.n_streams)
-        pos = np.empty(self.n_streams, dtype=np.uint64)
-        rc = _lib.acg_streams_positions(self._h, pos.ctypes.data)
+        a, ptr, k = self._ids(ids)
+        if a is not None and k == 0:
+            return np.empty(0, dtype=np.uint8), np.zeros(1, dtype=np.uint64)
+        out_offsets = np.empty((self.n_streams if a is None else k) + 1, dtype=np.uint64)
+        cnt = _u64()
+        rc = _lib.acg_streams_flush(self._h, ptr, k, None, 0, out_offsets.ctypes.data, C.byref(cnt))
+        while rc == E_OVERFLOW:  # the size query said how much; no stream was reset
+            out = np.empty(int(cnt.value), dtype=np.uint8)
+            rc = _lib.acg_streams_flush(self._h, ptr, k, out.ctypes.data, out.size, out_offsets.ctypes.data,
+                                        C.byref(cnt))
+            if rc == 0:
+                return out, out_offsets
         if rc:
             self._ac._raise(rc)
-        return pos
+        return np.empty(0, dtype=np.uint8), out_offsets
+
+    def flush(self, ids=None):
+        """The held bytes of the given streams (all when ids is None), one bytes object each; those streams then
+        restart from zero bytes."""
+        return self._split(*self.flush_np(ids))
+
+    def held(self):
+        """The bytes every stream holds back, uint64 [n_streams]: positions() - held() is its emit boundary."""
+        self._check(self.n_streams)
+        h = np.empty(self.n_streams, dtype=np.uint64)
+        rc = _lib.acg_streams_held(self._h, h.ctypes.data)
+        if rc:
+            self._ac._raise(rc)
+        return h
+
+    @staticmethod
+    def _split(values, offsets):
+        b, o = values.tobytes(), offsets.tolist()
+        return [b[o[i]:o[i + 1]] for i in range(len(o) - 1)]

@@ -114,6 +114,7 @@ struct Workspace {
   // a stream feed: the combined documents tail | chunk, their offsets and the chunk offsets given on the host
   DevBuf<uint8_t> d_sdocs;
   DevBuf<uint64_t> d_soffs;
+  DevBuf<uint64_t> d_held;  // a replace set's feed: the records of D with every stream's hold record
 };
 
 }  // namespace
@@ -152,12 +153,17 @@ struct acg_dfa {
 };
 
 // A stream set (acg_streams_create): the state of StreamLaunch (acb_device.cuh) on the automaton's device.
+// A replace set (acg_streams_create_replace) is a find_iter set that also holds its replacement table.
 struct acg_streams {
   const acg_dfa* a = nullptr;
   uint64_t n = 0, back = 0;
   bool overlapping = false;
+  bool replace = false;
   uint64_t* d_state = nullptr;  // [2 * n]: pos, then cursor
   uint8_t* d_tail = nullptr;    // [n * back]
+  // replace sets: the caller's rep_offsets [patterns_len + 1], the last one again (the empty replacement of the
+  // hold records, pid patterns_len), then the replacement bytes
+  uint64_t* d_rep = nullptr;
 };
 
 namespace {
@@ -1677,18 +1683,32 @@ bool replacements_ok(const acg_dfa* a, const BatchReplace& rp) {
   return rp.rep_bytes || rp.rep_offsets[rp.n_reps] == rp.rep_offsets[0];
 }
 
+// A batch's replacement table into w.d_rep: the offsets, then the bytes (replace_matches takes them from there).
+int upload_replacements(Workspace& w, const BatchReplace& rp) {
+  const uint64_t n_reps = rp.n_reps, rep_total = rp.rep_offsets[n_reps] - rp.rep_offsets[0];
+  int rc = w.d_rep.reserve(n_reps + 1 + (rep_total + 7) / 8);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(w.d_rep, rp.rep_offsets, (n_reps + 1) * 8, cudaMemcpyHostToDevice, w.stream));
+  if (rep_total)
+    CK(cudaMemcpyAsync(w.d_rep + n_reps + 1, rp.rep_bytes + rp.rep_offsets[0], rep_total, cudaMemcpyHostToDevice,
+                       w.stream));
+  return ACG_OK;
+}
+
 // The n find_iter matches of a batch -- the tuples `t` of the prefilter engine, in start order after the chain, or
-// (t.keys == nullptr) the records the sequential engine left at w.d_rec -- spliced with their replacements into
-// the output (ReplaceLaunch, acb_device.cuh).  `d_in`: the input at span_start, still being read.  Scratch: a_i
-// and e_i in the tuple buffers' keys, pids and documents in their pids, the deltas and their sum in w.d_scratch,
-// the tile index in w.d_temp.  Host output: the bytes in w.d_out and out_offsets in w.d_rec, copied to the caller
-// from there.  *out_len > cap: ACG_E_OVERFLOW, nothing written.
-int replace_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, int mode, uint64_t span_start,
-                    uint64_t span_end, const uint8_t* d_in, const uint64_t* d_offs, uint64_t n_docs,
-                    const BatchReplace& rp, bool dev_out, uint64_t cap, uint64_t* out_len) {
+// (t.keys == nullptr) the acg_doc_match records at `rec` -- spliced with their replacements into the output
+// (ReplaceLaunch, acb_device.cuh).  `d_in`: the input at span_start, still being read.  The table is on the device:
+// `rep_offsets` as the caller gave them, `rep_bytes` the bytes behind them.  Scratch: a_i and e_i in the tuple
+// buffers' keys, pids and documents in their pids, the deltas and their sum in w.d_scratch, the tile index in
+// w.d_temp.  Host output: the bytes in w.d_out and out_offsets in w.d_doc_incl (free once the search has run, and
+// not w.d_rec, which still holds a stream feed's records for its state step), copied to the caller from there.
+// *out_len > cap: ACG_E_OVERFLOW, nothing written.
+int replace_matches(const acg_dfa* a, const acb::TupleList& t, const uint64_t* rec, int sorted_buf, int mode,
+                    uint64_t span_start, uint64_t span_end, const uint8_t* d_in, const uint64_t* d_offs,
+                    uint64_t n_docs, const uint64_t* rep_offsets, const uint8_t* rep_bytes, const BatchReplace& rp,
+                    bool dev_out, uint64_t cap, uint64_t* out_len) {
   Workspace& w = cur_ws();
-  const uint64_t n = t.n, nd1 = n_docs + 1, n_reps = rp.n_reps;
-  const uint64_t rep_total = rp.rep_offsets[n_reps] - rp.rep_offsets[0];
+  const uint64_t n = t.n, nd1 = n_docs + 1;
   int rc;
   float ms = 0;
   // the time between ev2 and ev3, to order_ms
@@ -1699,20 +1719,15 @@ int replace_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, i
     w.stats.order_ms += ms;
     return ACG_OK;
   };
-  if ((rc = w.d_rep.reserve(n_reps + 1 + (rep_total + 7) / 8))) return rc;
-  CK(cudaMemcpyAsync(w.d_rep, rp.rep_offsets, (n_reps + 1) * 8, cudaMemcpyHostToDevice, w.stream));
-  if (rep_total)
-    CK(cudaMemcpyAsync(w.d_rep + n_reps + 1, rp.rep_bytes + rp.rep_offsets[0], rep_total, cudaMemcpyHostToDevice,
-                       w.stream));
   acb::ReplaceLaunch r{};
   r.t = t;
-  r.rec = t.keys ? nullptr : w.d_rec.p;
+  r.rec = t.keys ? nullptr : rec;
   r.mode = mode;
   r.span_start = span_start;
   r.doc_offsets = d_offs;
   r.n_docs = n_docs;
-  r.rep_offsets = w.d_rep;
-  r.rep_bytes = reinterpret_cast<const uint8_t*>(w.d_rep + n_reps + 1);
+  r.rep_offsets = rep_offsets;
+  r.rep_bytes = rep_bytes;
   r.in = d_in;
   uint64_t total = span_end - span_start;
   CK(cudaEventRecord(w.ev2, w.stream));
@@ -1744,9 +1759,9 @@ int replace_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, i
     r.out_offsets = rp.out_offsets;
   } else {
     if ((rc = w.d_out.reserve(std::max<uint64_t>(total, 1 << 20)))) return rc;
-    if ((rc = reserve_rec(w, (nd1 + 2) / 3))) return rc;  // 3 words per record: room for nd1 words
+    if ((rc = w.h_rec.reserve(nd1))) return rc;
     r.out = w.d_out;
-    r.out_offsets = w.d_rec;
+    r.out_offsets = reinterpret_cast<uint64_t*>(w.d_doc_incl.p);  // nd1 entries (reserve_docs)
   }
   const uint64_t n_tiles = total ? acb::replace_splice_tiles(r.out, total) : 0;
   if ((rc = w.d_temp.reserve(std::max<uint64_t>((n_tiles + 1) * 8, 16)))) return rc;
@@ -1774,13 +1789,46 @@ int replace_matches(const acg_dfa* a, const acb::TupleList& t, int sorted_buf, i
 
 // acg_streams_feed(_devout): the batch is the feed's combined documents D in the workspace (offsets on the device,
 // `docs_len` bytes), and its records become the feed's (StreamLaunch, acb_device.cuh).  `out` and `out_index` are
-// the caller's device arrays, or (`out_index` == nullptr) `out` is the caller's host array.
+// the caller's device arrays, or (!dev_out) `out` is the caller's host array.  acg_streams_replace_feed(_devout)
+// (`replace`, the set): `out` is the output bytes and `out_index` their offsets, both host arrays unless dev_out.
 struct BatchStreams {
   acb::StreamLaunch launch;  // the set, the chunks and D; the records and outputs are filled in by stream_records
   uint64_t docs_len;
-  uint64_t* out;
+  void* out;
   uint64_t* out_index;
+  bool dev_out;
+  const acg_streams* replace;
 };
+
+// A replace set's feed, once D is searched: the records of D and the hold records (launch_stream_hold), spliced
+// with the set's table into the feed's output, then the state of every stream.  *out_len > cap: ACG_E_OVERFLOW,
+// and nothing -- state included -- is written.
+int stream_replace(const acg_dfa* a, const BatchStreams& st, acb::StreamLaunch& p, uint64_t cap, uint64_t* out_len) {
+  Workspace& w = cur_ws();
+  const uint64_t n_rec = p.m + p.n;
+  int rc = w.d_held.reserve(std::max<uint64_t>(n_rec, 1 << 16) * 3);
+  if (rc) return rc;
+  p.held = w.d_held;
+  p.hold_pid = static_cast<uint32_t>(a->h.pattern_lens.size());
+  CK(acb::launch_stream_hold(p, w.stream));
+  w.stats.launches += 1;
+  const uint64_t* rep_offsets = st.replace->d_rep;
+  const uint8_t* rep_bytes = reinterpret_cast<const uint8_t*>(rep_offsets + p.hold_pid + 2);
+  const BatchReplace rp{nullptr, nullptr, p.hold_pid, static_cast<uint8_t*>(st.out), st.out_index};
+  if ((rc = replace_matches(a, acb::TupleList{nullptr, nullptr, nullptr, n_rec}, p.held, 0, 0, 0, p.docs_len, p.docs,
+                            reinterpret_cast<const uint64_t*>(p.doc_offsets), p.n, rep_offsets, rep_bytes, rp,
+                            st.dev_out, cap, out_len)))
+    return rc;
+  float ms = 0;
+  CK(cudaEventRecord(w.ev2, w.stream));
+  CK(acb::launch_stream_state(p, w.stream));
+  CK(cudaEventRecord(w.ev3, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+  w.stats.order_ms += ms;
+  w.stats.launches += 1;
+  return ACG_OK;
+}
 
 // The m records of D at `rec` with their index: the ones a previous feed has not returned (overlapping: those that
 // end after their tail), rebased and tagged, then the state of every stream.  ms_to gets the batch's time from ev2
@@ -1797,6 +1845,7 @@ int stream_records(const acg_dfa* a, const BatchStreams& st, const uint64_t* rec
   p.rec_index = rec_index;
   p.m = m;
   p.keep = nullptr;
+  if (st.replace) return stream_replace(a, st, p, cap, n_out);
   uint64_t kept = m;
   int rc;
   CK(cudaEventRecord(w.ev2, w.stream));
@@ -1816,9 +1865,9 @@ int stream_records(const acg_dfa* a, const BatchStreams& st, const uint64_t* rec
   *n_out = kept;
   if (kept > cap) return ACG_E_OVERFLOW;
   if (kept && !st.out) return ACG_E_INVALID_ARG;
-  const bool dev_out = st.out_index != nullptr;
+  const bool dev_out = st.dev_out;
   if (!dev_out && (rc = w.d_out.reserve(std::max<uint64_t>(kept * 24, 1 << 20)))) return rc;
-  p.out = dev_out ? st.out : reinterpret_cast<uint64_t*>(w.d_out.p);
+  p.out = dev_out ? static_cast<uint64_t*>(st.out) : reinterpret_cast<uint64_t*>(w.d_out.p);
   p.out_index = st.out_index;
   CK(acb::launch_stream_records(p, w.stream));
   CK(acb::launch_stream_state(p, w.stream));
@@ -1944,6 +1993,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
   }
   Placement pl;
   if ((rc = place_input(a, hay, hay_on_device, hay_len, span_start, span_end, use_pf, &pl))) return rc;
+  if (rp && (rc = upload_replacements(w, *rp))) return rc;
+  const uint64_t* rep_offsets = w.d_rep;
+  const uint8_t* rep_bytes = rp ? reinterpret_cast<const uint8_t*>(w.d_rep + rp->n_reps + 1) : nullptr;
   // The end of a batch: the time between ev2 and ev3 to `ms_to` -- the sequential engine's scan, the order time
   // of the prefilter engine's per-document step -- and for host output the copy of the flags and the records.
   auto finish = [&](float& ms_to) -> int {
@@ -2012,8 +2064,8 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
         return cover_matches(a, recs, 0, 0, what == kBatchFindIter, span_start, span_end, d_offs, n_docs, *cv,
                              dv != nullptr);
       if (rp)
-        return replace_matches(a, recs, 0, 0, span_start, span_end, pl.base + span_start, d_offs, n_docs, *rp,
-                               dv != nullptr, cap, n_out);
+        return replace_matches(a, recs, d_rec, 0, 0, span_start, span_end, pl.base + span_start, d_offs, n_docs,
+                               rep_offsets, rep_bytes, *rp, dv != nullptr, cap, n_out);
       return count_matches(a, recs, 0, 0, span_start, d_offs, n_docs, *co, dv != nullptr, cap, n_out);
     }
     // the CSR index is the inclusive scan behind a zero
@@ -2066,8 +2118,9 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
     return count_matches(a, tuple_list(a, w, r), r.sorted_buf, chain_mode, span_start, d_offs, n_docs, *co,
                          dv != nullptr, cap, n_out);
   if (rp)  // the chain's matches in start order: the splice's segments follow each other
-    return replace_matches(a, tuple_list(a, w, r), r.sorted_buf, chain_mode, span_start, span_end,
-                           pl.base + span_start, d_offs, n_docs, *rp, dv != nullptr, cap, n_out);
+    return replace_matches(a, tuple_list(a, w, r), nullptr, r.sorted_buf, chain_mode, span_start, span_end,
+                           pl.base + span_start, d_offs, n_docs, rep_offsets, rep_bytes, *rp, dv != nullptr, cap,
+                           n_out);
   *n_out = r.n;
   if ((rc = records(r.n))) return rc;
   CK(cudaEventRecord(w.ev2, w.stream));
@@ -2091,13 +2144,15 @@ int batch_impl(const acg_dfa* a, int what, const uint8_t* hay, bool hay_on_devic
 }
 
 // acg_streams_feed / acg_streams_feed_devout (include/acb200.h).  dev_out: `out` and `match_offsets` are device
-// arrays, else `out` is a host array.  The chunk offsets are checked (on the device when they are there) and D's
+// arrays, else `out` is a host array.  With `replace`, acg_streams_replace_feed(_devout): `out` is the output bytes
+// and `match_offsets` their offsets, both host arrays unless dev_out.  The chunk offsets are checked (on the device when they are there) and D's
 // length fetched in one round trip; D is gathered, searched by batch_impl and its records finished by
 // stream_records.  Staging and gather time go to h2d_ms.
 int streams_feed_impl(acg_streams* set, const uint8_t* hay, bool hay_on_device, uint64_t hay_len,
-                      const uint64_t* chunk_offsets, bool offsets_on_device, uint64_t n_streams, uint64_t* out,
-                      uint64_t cap, uint64_t* match_offsets, bool dev_out, uint64_t* n_out) {
-  if (!set || !chunk_offsets || !n_out || n_streams != set->n || (dev_out && !match_offsets) || (!out && cap))
+                      const uint64_t* chunk_offsets, bool offsets_on_device, uint64_t n_streams, void* out,
+                      uint64_t cap, uint64_t* match_offsets, bool dev_out, bool replace, uint64_t* n_out) {
+  if (!set || set->replace != replace || !chunk_offsets || !n_out || n_streams != set->n ||
+      ((dev_out || replace) && !match_offsets) || (!out && cap))
     return ACG_E_INVALID_ARG;
   *n_out = 0;
   const uint64_t n = set->n, n1 = n + 1;
@@ -2161,10 +2216,52 @@ int streams_feed_impl(acg_streams* set, const uint8_t* hay, bool hay_on_device, 
   float ms = 0;
   cudaEventElapsedTime(&ms, w.ev0, w.ev1);
   w.stats.h2d_ms = ms;
-  BatchStreams st{p, p.docs_len, out, dev_out ? match_offsets : nullptr};
+  BatchStreams st{p, p.docs_len, out, dev_out || replace ? match_offsets : nullptr, dev_out, replace ? set : nullptr};
   return batch_impl(a, set->overlapping ? kBatchOverlapping : kBatchFindIter, p.docs, true, p.docs_len,
                     w.d_soffs, n, 0, reinterpret_cast<acg_match*>(out), cap, n_out, nullptr, 0, nullptr, nullptr,
                     nullptr, nullptr, &st);
+}
+
+// acg_streams_create, and with `rp` (its table only) acg_streams_create_replace.
+int streams_create(const acg_dfa* a, uint64_t n_streams, int overlapping, const BatchReplace* rp, acg_streams** out) {
+  if (!a || !out || n_streams == 0 || n_streams >= (1ull << 32)) return ACG_E_INVALID_ARG;
+  *out = nullptr;
+  // StreamChunkIter::new, src/automaton.rs:1087-1103, and try_find_overlapping_iter, :397-423
+  if (a->h.match_kind != ACG_STANDARD) return overlapping ? ACG_E_UNSUPPORTED_OVERLAPPING : ACG_E_UNSUPPORTED_STREAM;
+  if (a->has_empty) return ACG_E_UNSUPPORTED_EMPTY;
+  int rc = check_anchored(a->h.start_kind, 0);
+  if (rc || (rc = check_start(a->h, 0))) return rc;
+  if (rp && !replacements_ok(a, *rp)) return ACG_E_INVALID_ARG;
+  if (!a->on_device) return ACG_E_NO_DEVICE;
+  acg_streams* s = new (std::nothrow) acg_streams();
+  if (!s) return ACG_E_NOMEM;
+  s->a = a;
+  s->n = n_streams;
+  s->back = a->h.max_pattern_len ? a->h.max_pattern_len - 1 : 0;
+  s->overlapping = overlapping != 0;
+  s->replace = rp != nullptr;
+  DeviceGuard guard(a->device);
+  cudaError_t e = cudaMalloc(&s->d_state, n_streams * 16);
+  if (e != cudaSuccess) s->d_state = nullptr;
+  if (e == cudaSuccess && (e = cudaMalloc(&s->d_tail, std::max<uint64_t>(n_streams * s->back, 16))) != cudaSuccess)
+    s->d_tail = nullptr;
+  if (e == cudaSuccess) e = cudaMemset(s->d_state, 0, n_streams * 16);
+  if (e == cudaSuccess && rp) {
+    const uint64_t n_reps = rp->n_reps, rep_total = rp->rep_offsets[n_reps] - rp->rep_offsets[0];
+    std::vector<uint64_t> offs(rp->rep_offsets, rp->rep_offsets + n_reps + 1);
+    offs.push_back(offs.back());
+    if ((e = cudaMalloc(&s->d_rep, (n_reps + 2) * 8 + rep_total)) != cudaSuccess) s->d_rep = nullptr;
+    if (e == cudaSuccess) e = cudaMemcpy(s->d_rep, offs.data(), (n_reps + 2) * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && rep_total)
+      e = cudaMemcpy(s->d_rep + n_reps + 2, rp->rep_bytes + rp->rep_offsets[0], rep_total, cudaMemcpyHostToDevice);
+  }
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    acg_streams_free(s);
+    return e == cudaErrorMemoryAllocation ? ACG_E_NOMEM : ACG_E_CUDA;
+  }
+  *out = s;
+  return ACG_OK;
 }
 
 }  // namespace
@@ -2617,33 +2714,13 @@ int acg_replace_all_batch_devout(const acg_dfa* a, const void* d_hay, uint64_t h
 }
 
 int acg_streams_create(const acg_dfa* a, uint64_t n_streams, int overlapping, acg_streams** out) {
-  if (!a || !out || n_streams == 0 || n_streams >= (1ull << 32)) return ACG_E_INVALID_ARG;
-  *out = nullptr;
-  // StreamChunkIter::new, src/automaton.rs:1087-1103, and try_find_overlapping_iter, :397-423
-  if (a->h.match_kind != ACG_STANDARD) return overlapping ? ACG_E_UNSUPPORTED_OVERLAPPING : ACG_E_UNSUPPORTED_STREAM;
-  if (a->has_empty) return ACG_E_UNSUPPORTED_EMPTY;
-  int rc = check_anchored(a->h.start_kind, 0);
-  if (rc || (rc = check_start(a->h, 0))) return rc;
-  if (!a->on_device) return ACG_E_NO_DEVICE;
-  acg_streams* s = new (std::nothrow) acg_streams();
-  if (!s) return ACG_E_NOMEM;
-  s->a = a;
-  s->n = n_streams;
-  s->back = a->h.max_pattern_len ? a->h.max_pattern_len - 1 : 0;
-  s->overlapping = overlapping != 0;
-  DeviceGuard guard(a->device);
-  cudaError_t e = cudaMalloc(&s->d_state, n_streams * 16);
-  if (e != cudaSuccess) s->d_state = nullptr;
-  if (e == cudaSuccess && (e = cudaMalloc(&s->d_tail, std::max<uint64_t>(n_streams * s->back, 16))) != cudaSuccess)
-    s->d_tail = nullptr;
-  if (e == cudaSuccess) e = cudaMemset(s->d_state, 0, n_streams * 16);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    acg_streams_free(s);
-    return e == cudaErrorMemoryAllocation ? ACG_E_NOMEM : ACG_E_CUDA;
-  }
-  *out = s;
-  return ACG_OK;
+  return streams_create(a, n_streams, overlapping, nullptr, out);
+}
+
+int acg_streams_create_replace(const acg_dfa* a, uint64_t n_streams, const uint8_t* rep_bytes,
+                               const uint64_t* rep_offsets, uint64_t n_reps, acg_streams** out) {
+  const BatchReplace rp{rep_bytes, rep_offsets, n_reps, nullptr, nullptr};
+  return streams_create(a, n_streams, 0, &rp, out);
 }
 
 void acg_streams_free(acg_streams* s) {
@@ -2652,6 +2729,7 @@ void acg_streams_free(acg_streams* s) {
     DeviceGuard guard(s->a->device);
     cudaFree(s->d_state);
     cudaFree(s->d_tail);
+    cudaFree(s->d_rep);
   }
   delete s;
 }
@@ -2683,16 +2761,84 @@ int acg_streams_positions(const acg_streams* s, uint64_t* pos) {
 int acg_streams_feed(acg_streams* s, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
                      const uint64_t* chunk_offsets, uint64_t n_streams, acg_doc_match* out, uint64_t cap,
                      uint64_t* n_out) {
-  return streams_feed_impl(s, hay, hay_on_device != 0, hay_len, chunk_offsets, false, n_streams,
-                           reinterpret_cast<uint64_t*>(out), cap, nullptr, false, n_out);
+  return streams_feed_impl(s, hay, hay_on_device != 0, hay_len, chunk_offsets, false, n_streams, out, cap, nullptr,
+                           false, false, n_out);
 }
 
 int acg_streams_feed_devout(acg_streams* s, const void* d_hay, uint64_t hay_len, const uint64_t* chunk_offsets,
                             int offsets_on_device, uint64_t n_streams, acg_doc_match* d_out, uint64_t cap,
                             uint64_t* d_match_offsets, uint64_t* n_out) {
   return streams_feed_impl(s, static_cast<const uint8_t*>(d_hay), true, hay_len, chunk_offsets,
-                           offsets_on_device != 0, n_streams, reinterpret_cast<uint64_t*>(d_out), cap,
-                           d_match_offsets, true, n_out);
+                           offsets_on_device != 0, n_streams, d_out, cap, d_match_offsets, true, false, n_out);
+}
+
+int acg_streams_replace_feed(acg_streams* s, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                             const uint64_t* chunk_offsets, uint64_t n_streams, uint8_t* out, uint64_t cap,
+                             uint64_t* out_offsets, uint64_t* out_len) {
+  return streams_feed_impl(s, hay, hay_on_device != 0, hay_len, chunk_offsets, false, n_streams, out, cap,
+                           out_offsets, false, true, out_len);
+}
+
+int acg_streams_replace_feed_devout(acg_streams* s, const void* d_hay, uint64_t hay_len,
+                                    const uint64_t* chunk_offsets, int offsets_on_device, uint64_t n_streams,
+                                    uint8_t* d_out, uint64_t cap, uint64_t* d_out_offsets, uint64_t* out_len) {
+  return streams_feed_impl(s, static_cast<const uint8_t*>(d_hay), true, hay_len, chunk_offsets,
+                           offsets_on_device != 0, n_streams, d_out, cap, d_out_offsets, true, true, out_len);
+}
+
+int acg_streams_held(const acg_streams* s, uint64_t* held) {
+  if (!s || !s->replace || !held) return ACG_E_INVALID_ARG;
+  std::vector<uint64_t> st(2 * s->n);
+  DeviceGuard guard(s->a->device);
+  CK(cudaMemcpy(st.data(), s->d_state, s->n * 16, cudaMemcpyDeviceToHost));
+  for (uint64_t i = 0; i < s->n; ++i) held[i] = std::min(s->back, st[i] - st[s->n + i]);
+  return ACG_OK;
+}
+
+// The held bytes of the listed streams are their tails (L_s = held_s): their lengths and offsets are worked out on
+// the host from the state, and one kernel gathers the tails and zeroes the state.
+int acg_streams_flush(acg_streams* s, const uint64_t* ids, uint64_t n_ids, uint8_t* out, uint64_t cap,
+                      uint64_t* out_offsets, uint64_t* out_len) {
+  if (!s || !s->replace || !out_offsets || !out_len || (!out && cap)) return ACG_E_INVALID_ARG;
+  const uint64_t n = s->n, k = ids ? n_ids : n;
+  if (ids) {
+    std::vector<uint8_t> seen(n, 0);
+    for (uint64_t i = 0; i < n_ids; ++i)
+      if (ids[i] >= n || seen[ids[i]]++) return ACG_E_INVALID_ARG;
+  }
+  *out_len = 0;
+  const acg_dfa* a = s->a;
+  DeviceGuard guard(a->device);
+  std::vector<uint64_t> st(2 * n), offs(k + 1, 0);
+  CK(cudaMemcpy(st.data(), s->d_state, n * 16, cudaMemcpyDeviceToHost));
+  for (uint64_t j = 0; j < k; ++j) {
+    const uint64_t i = ids ? ids[j] : j;
+    offs[j + 1] = offs[j] + std::min(s->back, st[i] - st[n + i]);
+  }
+  const uint64_t total = offs[k];
+  *out_len = total;
+  if (total > cap) return ACG_E_OVERFLOW;
+  if (k) {
+    WsLease lease(a);
+    if (lease.rc) return lease.rc;
+    Workspace& w = cur_ws();
+    int rc = w.d_soffs.reserve(2 * k + 1);
+    if (rc || (rc = w.d_out.reserve(std::max<uint64_t>(total, 1 << 20)))) return rc;
+    acb::StreamLaunch p{};
+    p.n = n;
+    p.back = s->back;
+    p.pos = s->d_state;
+    p.cursor = s->d_state + n;
+    p.tail = s->d_tail;
+    uint64_t* d_ids = w.d_soffs + (k + 1);
+    CK(cudaMemcpyAsync(w.d_soffs, offs.data(), (k + 1) * 8, cudaMemcpyHostToDevice, w.stream));
+    if (ids) CK(cudaMemcpyAsync(d_ids, ids, k * 8, cudaMemcpyHostToDevice, w.stream));
+    CK(acb::launch_stream_flush(p, ids ? d_ids : nullptr, k, w.d_soffs, w.d_out, w.stream));
+    if (total && (rc = copy_to_host(a, out, w.d_out, total))) return rc;
+    CK(cudaStreamSynchronize(w.stream));
+  }
+  std::copy(offs.begin(), offs.end(), out_offsets);
+  return ACG_OK;
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

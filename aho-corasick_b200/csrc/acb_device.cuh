@@ -264,6 +264,10 @@ cudaError_t launch_replace_splice(const ReplaceLaunch& r, cudaStream_t s);
 //   launch_stream_records  the kept records at out[j * 3], rebased to stream offsets (+ pos - L_s), and out_index
 //   launch_stream_state    pos, cursor and the new tail: D_s[t - (pos - L_s) ..) with t = max(pos' - back, cursor')
 // Nothing before launch_stream_state writes the state, so a feed that stops before it leaves every stream as it was.
+// A replace set (find_iter mode) splices D instead of returning records: launch_stream_hold writes the records of D
+// with one more record after each stream's, [t - (pos - L_s), |D_s|) with the pid `hold_pid`, whose replacement is
+// empty; replacing them all (ReplaceLaunch) emits D_s up to the new tail start t, the emit boundary, and holds back
+// the new tail.  Stream s's records move by s places: record i of D to i + s, the hold record to rec_index[s + 1] + s.
 struct StreamLaunch {
   uint64_t n;                       // streams
   uint64_t back;                    // max_pattern_len - 1: the tail stride
@@ -282,12 +286,20 @@ struct StreamLaunch {
   unsigned long long* keep;         // overlapping: [m]; nullptr: every record is kept
   uint64_t* out;                    // [kept * 3]
   uint64_t* out_index;              // [n + 1] or nullptr
+  uint64_t* held;                   // replace sets: [(m + n) * 3] the records with each stream's hold record
+  uint32_t hold_pid;                // replace sets: patterns_len, the pid of the empty replacement
 };
 cudaError_t launch_stream_docs(const StreamLaunch& p, cudaStream_t s);
 cudaError_t launch_stream_gather(const StreamLaunch& p, cudaStream_t s);  // docs_len > 0
 cudaError_t launch_stream_keep(const StreamLaunch& p, cudaStream_t s);    // m > 0
 cudaError_t launch_stream_records(const StreamLaunch& p, cudaStream_t s);
 cudaError_t launch_stream_state(const StreamLaunch& p, cudaStream_t s);
+cudaError_t launch_stream_hold(const StreamLaunch& p, cudaStream_t s);
+// Flush of a replace set: the tail of stream ids[k] (k when ids is nullptr), out_offsets[k + 1] - out_offsets[k]
+// bytes, copied to out[out_offsets[k] ..), and that stream's pos and cursor zeroed.  n_ids > 0; ids hold no
+// duplicates.
+cudaError_t launch_stream_flush(const StreamLaunch& p, const uint64_t* ids, uint64_t n_ids,
+                                const uint64_t* out_offsets, uint8_t* out, cudaStream_t s);
 
 // Offsets in device memory: result[0] = 1 if some offs[i] > offs[i + 1] or offs[n_docs] > hay_len (left as it
 // was otherwise: the caller clears it), result[1] = offs[0], result[2] = offs[n_docs].

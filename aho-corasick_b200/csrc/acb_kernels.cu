@@ -26,6 +26,9 @@
 //        stream_keep_kernel       and every stream's new position, cursor and tail
 //        stream_records_kernel
 //        stream_state_kernel
+//        stream_hold_kernel       a replace set's feed: the records of D with each stream's held bytes as a
+//                                 deletion after them, for the replace kernels to splice
+//        stream_flush_kernel      a replace set's flush: the listed streams' tails out, their state zeroed
 //        check_offsets_kernel     validation of document offsets in device memory
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
@@ -747,20 +750,35 @@ __global__ void stream_records_kernel(StreamLaunch p) {
   }
 }
 
+// Stream s after the feed, from the records of D: its position pos' = base + |D_s| (base = pos - L_s, where D_s
+// starts), its cursor' and the start of its new tail t = max(pos' - back, cursor'), which is also a replace set's
+// emit boundary.  The state kernel and the hold kernel both take t from here, so the tail a replace feed holds back
+// is the one the state keeps.
+struct StreamNext {
+  uint64_t base, pos, cursor, t;
+};
+__device__ __forceinline__ StreamNext stream_next(const StreamLaunch& p, uint64_t s) {
+  StreamNext x;
+  x.base = p.pos[s] - stream_tail_len(p, s);
+  x.pos = x.base + (p.doc_offsets[s + 1] - p.doc_offsets[s]);
+  x.cursor = p.cursor[s];
+  if (!p.overlapping) {
+    const uint64_t lo = p.rec_index[s], hi = p.rec_index[s + 1];
+    if (hi > lo) x.cursor = x.base + p.rec[(hi - 1) * 3 + 2];
+  }
+  x.t = x.pos > p.back ? x.pos - p.back : 0;
+  if (x.cursor > x.t) x.t = x.cursor;
+  return x;
+}
+
 // One warp per stream: every lane reads the old state, then the new tail is copied and lane 0 stores pos and cursor.
 __global__ void stream_state_kernel(StreamLaunch p) {
   const uint64_t s = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint32_t lane = threadIdx.x & 31;
   if (s >= p.n) return;
   const uint64_t d0 = p.doc_offsets[s];
-  const uint64_t base = p.pos[s] - stream_tail_len(p, s), pos = base + (p.doc_offsets[s + 1] - d0);
-  uint64_t cursor = p.cursor[s];
-  if (!p.overlapping) {
-    const uint64_t lo = p.rec_index[s], hi = p.rec_index[s + 1];
-    if (hi > lo) cursor = base + p.rec[(hi - 1) * 3 + 2];
-  }
-  uint64_t t = pos > p.back ? pos - p.back : 0;
-  if (cursor > t) t = cursor;
+  const StreamNext x = stream_next(p, s);
+  const uint64_t base = x.base, pos = x.pos, cursor = x.cursor, t = x.t;
   const uint8_t* src = p.docs + d0 + (t - base);
   uint8_t* dst = p.tail + s * p.back;
   for (uint64_t k = lane; k < pos - t; k += 32) dst[k] = src[k];
@@ -768,6 +786,42 @@ __global__ void stream_state_kernel(StreamLaunch p) {
   if (lane == 0) {
     p.pos[s] = pos;
     p.cursor[s] = cursor;
+  }
+}
+
+// Thread i < m: record i of D, moved past the hold records of the streams before its own; thread s < n: stream s's
+// hold record [t - base, |D_s|) after its last record.  D's find_iter records all end at or before cursor' <= t, so
+// the list stays in start order within every stream.
+__global__ void stream_hold_kernel(StreamLaunch p) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < p.m) {
+    const uint64_t* r = p.rec + i * 3;
+    uint64_t* q = p.held + (i + (r[0] >> 32)) * 3;
+    q[0] = r[0];
+    q[1] = r[1];
+    q[2] = r[2];
+  }
+  if (i < p.n) {
+    const StreamNext x = stream_next(p, i);
+    uint64_t* q = p.held + (p.rec_index[i + 1] + i) * 3;
+    q[0] = (i << 32) | p.hold_pid;
+    q[1] = x.t - x.base;
+    q[2] = x.pos - x.base;
+  }
+}
+
+// One warp per listed stream: its tail to the output, then lane 0 zeroes its state.
+__global__ void stream_flush_kernel(StreamLaunch p, const uint64_t* ids, uint64_t n_ids, const uint64_t* out_offsets,
+                                    uint8_t* out) {
+  const uint64_t k = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31;
+  if (k >= n_ids) return;
+  const uint64_t s = ids ? ids[k] : k, o = out_offsets[k], len = out_offsets[k + 1] - o;
+  const uint8_t* src = p.tail + s * p.back;
+  for (uint64_t j = lane; j < len; j += 32) out[o + j] = src[j];
+  if (lane == 0) {
+    p.pos[s] = 0;
+    p.cursor[s] = 0;
   }
 }
 
@@ -970,6 +1024,18 @@ cudaError_t launch_stream_records(const StreamLaunch& p, cudaStream_t s) {
 
 cudaError_t launch_stream_state(const StreamLaunch& p, cudaStream_t s) {
   ACB_LAUNCH(stream_state_kernel, (unsigned)((p.n * 32 + 255) / 256), 256, 0, s, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_hold(const StreamLaunch& p, cudaStream_t s) {
+  const uint64_t n = p.m > p.n ? p.m : p.n;
+  ACB_LAUNCH(stream_hold_kernel, (unsigned)((n + 255) / 256), 256, 0, s, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_flush(const StreamLaunch& p, const uint64_t* ids, uint64_t n_ids,
+                                const uint64_t* out_offsets, uint8_t* out, cudaStream_t s) {
+  ACB_LAUNCH(stream_flush_kernel, (unsigned)((n_ids * 32 + 255) / 256), 256, 0, s, p, ids, n_ids, out_offsets, out);
   return cudaGetLastError();
 }
 

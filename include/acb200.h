@@ -381,6 +381,49 @@ int acg_streams_feed_devout(acg_streams* set, const void* d_hay, uint64_t hay_le
                             int offsets_on_device, uint64_t n_streams, acg_doc_match* d_out, uint64_t cap,
                             uint64_t* d_match_offsets, uint64_t* n_out);
 
+/* ---- replace sets: try_stream_replace_all over many streams, spliced on the device ----------
+ * A replace set is a find_iter stream set that writes text instead of records.  For stream s let
+ * X_s be the bytes it has received since creation, its last reset or its last flush, pos_s = |X_s|,
+ * c_s the end of the last find_iter match of X_s (0 if none), and h_s = max(c_s, pos_s -
+ * (max_pattern_len - 1)), floored at 0: the emit boundary.  Everything before h_s is settled; the
+ * held bytes X_s[h_s, pos_s), at most max_pattern_len - 1 of them, hold no match yet.
+ * acg_streams_create_replace: the checks of acg_streams_create in find_iter mode, in its order, then
+ * the replacement table as acg_replace_all_batch checks it (one per pattern, offsets that do not
+ * decrease, rep_bytes non-NULL when there are bytes; else ACG_E_INVALID_ARG), then ACG_E_NOMEM.  The
+ * table is copied to the device; the caller's arrays are not kept.
+ * acg_streams_replace_feed(_devout): a feed in the form of acg_streams_feed(_devout) that takes stream
+ * s from (pos, h) to (pos', h') writes X_s[h, h') with every find_iter match of X_s in that range
+ * replaced by its pattern's replacement (empty ones delete; replacements are not searched again):
+ * stream s's bytes are out[out_offsets[s] .. out_offsets[s + 1]), out_offsets[n_streams + 1],
+ * out_offsets[0] = 0, *out_len = out_offsets[n_streams].  Every match lies wholly inside or outside
+ * that range.  So a stream's outputs over all its feeds, followed by its flush, are
+ * replace_all_bytes(X_s), what try_stream_replace_all writes for X_s.  The output is bytes: h may
+ * split a multi-byte UTF-8 character between one feed's output and the next.  *out_len > cap
+ * returns ACG_E_OVERFLOW with the required size, writes nothing and changes no stream.  The other
+ * errors, their order and the offset rules are those of acg_streams_feed(_devout); a NULL
+ * out_offsets is ACG_E_INVALID_ARG.  _devout: out and out_offsets are device pointers.  out must not
+ * overlap the chunks.
+ * acg_streams_flush: for each id in ids (ids == NULL: every stream, in order) the stream's held
+ * bytes X_s[h, pos), raw, in the same CSR form into host memory (n_ids + 1 or n_streams + 1
+ * offsets); those streams then restart from zero bytes.  An id >= n_streams, a duplicate id, a NULL
+ * out_offsets or out_len, or a NULL out with cap > 0 gives ACG_E_INVALID_ARG and touches no stream;
+ * *out_len > cap gives ACG_E_OVERFLOW with the required size and resets no stream.
+ * acg_streams_held: held[s] = pos_s - h_s, held in host memory with n_streams entries.
+ * acg_streams_positions, acg_streams_reset (which discards the held bytes unemitted) and
+ * acg_streams_free take replace sets.  acg_streams_feed(_devout) on a replace set, and the calls
+ * above on another set, give ACG_E_INVALID_ARG. */
+int acg_streams_create_replace(const acg_dfa* dfa, uint64_t n_streams, const uint8_t* rep_bytes,
+                               const uint64_t* rep_offsets, uint64_t n_reps, acg_streams** out);
+int acg_streams_replace_feed(acg_streams* set, const uint8_t* hay, int hay_on_device, uint64_t hay_len,
+                             const uint64_t* chunk_offsets, uint64_t n_streams, uint8_t* out, uint64_t cap,
+                             uint64_t* out_offsets, uint64_t* out_len);
+int acg_streams_replace_feed_devout(acg_streams* set, const void* d_hay, uint64_t hay_len,
+                                    const uint64_t* chunk_offsets, int offsets_on_device, uint64_t n_streams,
+                                    uint8_t* d_out, uint64_t cap, uint64_t* d_out_offsets, uint64_t* out_len);
+int acg_streams_flush(acg_streams* set, const uint64_t* ids, uint64_t n_ids, uint8_t* out, uint64_t cap,
+                      uint64_t* out_offsets, uint64_t* out_len);
+int acg_streams_held(const acg_streams* set, uint64_t* held);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

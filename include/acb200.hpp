@@ -627,6 +627,119 @@ class Streams {
   uint64_t cap_hint_ = 4096;
 };
 
+// A replace set (acg_streams_create_replace, include/acb200.h): n streams whose text is replaced on the device as
+// their bytes arrive.  feed() takes one chunk per stream -- CSR `offsets` [n + 1] into `chunks` -- and returns per
+// stream the text this feed settled, with every find_iter match replaced by replacements[pattern]; flush() returns
+// the bytes the streams still hold back and restarts them.  A stream's feeds followed by its flush give
+// replace_all_bytes of everything it received.  The automaton must outlive the set; one call at a time per set.
+class ReplaceStreams {
+ public:
+  template <class Replacements>
+  ReplaceStreams(const AhoCorasick& ac, uint64_t n_streams, const Replacements& replacements) {
+    std::string table;
+    std::vector<uint64_t> at{0};
+    for (const auto& x : replacements) {
+      table.append(std::string_view(x));
+      at.push_back(table.size());
+    }
+    Result<int> r;
+    r.error = acg_streams_create_replace(ac.raw(), n_streams, reinterpret_cast<const uint8_t*>(table.data()),
+                                         at.data(), at.size() - 1, &h_);
+    r.unwrap();
+    n_ = n_streams;
+  }
+  ReplaceStreams(ReplaceStreams&& o) noexcept : h_(o.h_), n_(o.n_) { o.h_ = nullptr; }
+  ReplaceStreams& operator=(ReplaceStreams&& o) noexcept {
+    if (this != &o) { close(); h_ = o.h_; n_ = o.n_; o.h_ = nullptr; }
+    return *this;
+  }
+  ReplaceStreams(const ReplaceStreams&) = delete;
+  ReplaceStreams& operator=(const ReplaceStreams&) = delete;
+  ~ReplaceStreams() { close(); }
+
+  uint64_t n_streams() const { return n_; }
+
+  Result<std::vector<std::string>> try_feed(std::string_view chunks, const std::vector<uint64_t>& offsets) {
+    const uint64_t n_chunks = offsets.empty() ? 0 : offsets.size() - 1;
+    const uint64_t span = offsets.empty() ? 0 : offsets.back() - offsets.front();
+    return collect(span + span / 8 + 4096, [&](uint8_t* out, uint64_t cap, uint64_t* out_offs, uint64_t* need) {
+      return acg_streams_replace_feed(h_, reinterpret_cast<const uint8_t*>(chunks.data()), 0, chunks.size(),
+                                      offsets.empty() ? nullptr : offsets.data(), n_chunks, out, cap, out_offs, need);
+    }, n_);
+  }
+  std::vector<std::string> feed(std::string_view chunks, const std::vector<uint64_t>& offsets) {
+    return std::move(try_feed(chunks, offsets).unwrap());
+  }
+  // The held bytes of the given streams, raw, and those streams restarted from zero bytes; flush() takes every
+  // stream.
+  std::vector<std::string> flush(const std::vector<uint64_t>& ids) {
+    if (ids.empty()) return {};
+    return std::move(collect(0, [&](uint8_t* out, uint64_t cap, uint64_t* out_offs, uint64_t* need) {
+      return acg_streams_flush(h_, ids.data(), ids.size(), out, cap, out_offs, need);
+    }, ids.size()).unwrap());
+  }
+  std::vector<std::string> flush() {
+    return std::move(collect(0, [&](uint8_t* out, uint64_t cap, uint64_t* out_offs, uint64_t* need) {
+      return acg_streams_flush(h_, nullptr, 0, out, cap, out_offs, need);
+    }, n_).unwrap());
+  }
+  // Restart the given streams from zero bytes, discarding what they hold back; reset() restarts every stream.
+  void reset(const std::vector<uint64_t>& ids) {
+    if (ids.empty()) return;
+    Result<int> r;
+    r.error = acg_streams_reset(h_, ids.data(), ids.size());
+    r.unwrap();
+  }
+  void reset() {
+    Result<int> r;
+    r.error = acg_streams_reset(h_, nullptr, 0);
+    r.unwrap();
+  }
+  // The bytes every stream has received.
+  std::vector<uint64_t> positions() const {
+    std::vector<uint64_t> pos(n_);
+    Result<int> r;
+    r.error = acg_streams_positions(h_, pos.data());
+    r.unwrap();
+    return pos;
+  }
+  // The bytes every stream holds back: positions() - held() is where its output has reached.
+  std::vector<uint64_t> held() const {
+    std::vector<uint64_t> h(n_);
+    Result<int> r;
+    r.error = acg_streams_held(h_, h.data());
+    r.unwrap();
+    return h;
+  }
+  acg_streams* raw() const { return h_; }
+
+ private:
+  // The two-call protocol in output bytes: `call(out, cap, out_offsets, &need)` until it fits, split per entry.
+  template <class Call>
+  static Result<std::vector<std::string>> collect(uint64_t cap, Call call, uint64_t n_out) {
+    Result<std::vector<std::string>> r;
+    std::string bytes;
+    std::vector<uint64_t> offs(n_out + 1);
+    uint64_t need = 0;
+    for (;; cap = need) {
+      bytes.resize(cap);
+      r.error = call(reinterpret_cast<uint8_t*>(bytes.data()), cap, offs.data(), &need);
+      if (r.error != ACG_E_OVERFLOW) break;
+    }
+    if (r.error == 0) {
+      r.value.reserve(n_out);
+      for (uint64_t i = 0; i < n_out; ++i) r.value.emplace_back(bytes.substr(offs[i], offs[i + 1] - offs[i]));
+    }
+    return r;
+  }
+  void close() {
+    if (h_) acg_streams_free(h_);
+    h_ = nullptr;
+  }
+  acg_streams* h_ = nullptr;
+  uint64_t n_ = 0;
+};
+
 template <class Patterns>
 AhoCorasick AhoCorasickBuilder::build(const Patterns& patterns) const {
   std::vector<const uint8_t*> ptrs;
