@@ -182,6 +182,11 @@ def _declare(lib):
                                                     C.POINTER(_u64)]
     lib.acg_streams_flush.argtypes = [_vp, _vp, _u64, _vp, _u64, _vp, C.POINTER(_u64)]
     lib.acg_streams_held.argtypes = [_vp, _vp]
+    lib.acg_candidates_create.argtypes = [_vp, _vp, _vp, _u64, C.POINTER(_vp)]
+    lib.acg_candidates_free.argtypes = [_vp]
+    lib.acg_candidates_free.restype = None
+    lib.acg_streams_lookahead.argtypes = [_vp, _vp, _vp, _u64, _vp]
+    lib.acg_streams_lookahead_devout.argtypes = [_vp, _vp, _vp, _u64, _vp]
     lib.acg_device_count.argtypes = []
     # multi-GPU (include/acb200.h, SURVEY.md section 8e)
     lib.acg_comm_unique_id.argtypes = [_vp]
@@ -1202,6 +1207,11 @@ class AhoCorasick:
         followed by its flush, are replace_all_bytes of everything it received, as stream_replace_all writes it."""
         return ReplaceStreams(self, n_streams, replace_with)
 
+    def candidates(self, cands):
+        """A fixed list of candidate chunks on the device (acg_candidates_create) -- a list of bytes / str, or
+        (values, offsets) as the batch calls take -- for the lookahead of this automaton's stream sets."""
+        return Candidates(self, cands)
+
     def try_stream_replace_all_with(self, rdr, wtr, replace_with, chunk_bytes=64 << 20):
         """`try_stream_replace_all_with`, src/ahocorasick.rs:1807 -> src/automaton.rs:601-636:
         `replace_with(match, matched bytes, wtr)` writes the replacement; text between matches is
@@ -1264,7 +1274,7 @@ class AhoCorasick:
 
 
 class _StreamSet:
-    """What every stream set (Streams, ReplaceStreams) has: its handle, its life cycle, reset and positions."""
+    """What every stream set (Streams, ReplaceStreams) has: handle, life cycle, reset, positions, lookahead."""
 
     def close(self):
         if self._h and _lib is not None:
@@ -1318,6 +1328,82 @@ class _StreamSet:
         if rc:
             self._ac._raise(rc)
         return pos
+
+    def _look(self, cands, ids):
+        if not self._h:
+            raise ValueError("the stream set is closed")
+        if not isinstance(cands, Candidates) or not cands._h or cands._ac is not self._ac:
+            raise ValueError("lookahead takes an open Candidates of this set's automaton")
+        a, ptr, n = self._ids(ids)
+        return a, ptr, n, (self.n_streams if a is None else n)
+
+    def lookahead_np(self, cands, ids=None):
+        """For every row -- stream ids[k], or every stream when ids is None -- and every candidate c of `cands`
+        (AhoCorasick.candidates): whether feeding that stream c would return a match, as a bool array
+        [rows, len(cands)].  No stream changes."""
+        a, ptr, n, rows = self._look(cands, ids)
+        out = np.empty((rows, cands.n), dtype=np.bool_)
+        if rows == 0:  # an empty id list: no call, whose NULL ids would mean every stream
+            return out
+        rc = _lib.acg_streams_lookahead(self._h, cands._h, ptr, n, out.ctypes.data if out.size else None)
+        if rc:
+            self._ac._raise(rc)
+        return out
+
+    def lookahead_torch(self, cands, ids=None, device=None):
+        """lookahead_np as a CUDA torch.bool tensor on the automaton's device (`device`, by default the current
+        CUDA device).  Torch's current stream is synchronised first, as feed_torch does."""
+        import torch
+        a, ptr, n, rows = self._look(cands, ids)
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        out = torch.empty((rows, cands.n), dtype=torch.bool, device=dev)
+        if rows == 0:
+            return out
+        torch.cuda.current_stream(dev).synchronize()
+        rc = _lib.acg_streams_lookahead_devout(self._h, cands._h, ptr, n, out.data_ptr() if out.numel() else None)
+        if rc:
+            self._ac._raise(rc)
+        return out
+
+
+class Candidates:
+    """A candidate set (include/acb200.h, acg_candidates_create): a fixed list of byte strings -- a tokenizer's
+    vocabulary, say -- copied once to the automaton's device and reused by every lookahead of that automaton's
+    stream sets.  Create it with AhoCorasick.candidates(); use it as a context manager or close() it."""
+
+    def __init__(self, ac, cands):
+        self._ac = ac
+        self._h = None
+        keep, ptr, _, on_dev, offs = _batch_input(cands)
+        if on_dev:
+            raise TypeError("candidates are given in host memory")
+        h = _vp()
+        rc = _lib.acg_candidates_create(ac._h, ptr if offs[-1] > offs[0] else None, offs.ctypes.data,
+                                        offs.size - 1, C.byref(h))
+        if rc:
+            ac._raise(rc)
+        self._h = h
+        self.n = int(offs.size - 1)
+
+    def __len__(self):
+        return self.n
+
+    def close(self):
+        if self._h and _lib is not None:
+            _lib.acg_candidates_free(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class Streams(_StreamSet):

@@ -166,6 +166,15 @@ struct acg_streams {
   uint64_t* d_rep = nullptr;
 };
 
+// A candidate set (acg_candidates_create) on the automaton's device: the offsets, from 0, and the bytes already mapped
+// through the automaton's byte classes, which is why it is bound to that automaton.
+struct acg_candidates {
+  const acg_dfa* a = nullptr;
+  uint64_t n = 0;
+  uint64_t* d_offs = nullptr;   // [n + 1]
+  uint8_t* d_classes = nullptr;  // [d_offs[n]]
+};
+
 namespace {
 
 // The workspace leased by the search running on this thread (WsLease below).
@@ -2264,6 +2273,92 @@ int streams_create(const acg_dfa* a, uint64_t n_streams, int overlapping, const 
   return ACG_OK;
 }
 
+// acg_streams_lookahead(_devout): the LookLaunch steps (acb_device.cuh) into `out` (dev_out) or into the workspace's
+// output buffer, copied to the host `out` from there.  Scratch: the tuple buffers (states and rows, sorted and not),
+// the per-document counts (run starts, then the run index), d_scratch (the run of every row) and d_soffs (the ids).
+// Nothing of the set is written.
+int streams_lookahead_impl(const acg_streams* set, const acg_candidates* c, const uint64_t* ids, uint64_t n_ids,
+                           uint8_t* out, bool dev_out) {
+  if (!set || !c || c->a != set->a) return ACG_E_INVALID_ARG;
+  const uint64_t n_rows = ids ? n_ids : set->n;
+  if (n_rows >= (1ull << 32)) return ACG_E_INVALID_ARG;
+  for (uint64_t i = 0; ids && i < n_ids; ++i)
+    if (ids[i] >= set->n) return ACG_E_INVALID_ARG;
+  const uint64_t total = n_rows * c->n;
+  if (total && !out) return ACG_E_INVALID_ARG;
+  if (!total) return ACG_OK;
+  const acg_dfa* a = set->a;
+  DeviceGuard guard(a->device);
+  WsLease lease(a);
+  if (lease.rc) return lease.rc;
+  Workspace& w = cur_ws();
+  int rc = reserve_tuples(w, std::max<uint64_t>(n_rows, 1 << 12));
+  if (rc || (rc = reserve_docs(w, n_rows)) || (rc = w.d_scratch.reserve(std::max<uint64_t>(n_rows, 1 << 12))) ||
+      (ids && (rc = w.d_soffs.reserve(n_rows))) || (!dev_out && (rc = w.d_out.reserve(total)))) {
+    cudaGetLastError();  // a failed allocation: the buffers are empty again, the error is not sticky
+    return ACG_E_NOMEM;
+  }
+  acb::LookLaunch p{};
+  p.st.n = set->n;
+  p.st.back = set->back;
+  p.st.overlapping = set->overlapping;
+  p.st.pos = set->d_state;
+  p.st.cursor = set->d_state + set->n;
+  p.st.tail = set->d_tail;
+  p.ids = ids ? w.d_soffs.p : nullptr;
+  p.n_rows = n_rows;
+  p.cand_offsets = c->d_offs;
+  p.cand_classes = c->d_classes;
+  p.n_cands = c->n;
+  p.keys = w.d_keys[0];
+  p.rows = w.d_pids[0];
+  p.skeys = w.d_keys[1];
+  p.srows = w.d_pids[1];
+  p.heads = w.d_doc_counts;
+  p.row_u = w.d_scratch;
+  p.out = dev_out ? out : w.d_out.p;
+  p.sm_count = 132;
+  cudaDeviceGetAttribute(&p.sm_count, cudaDevAttrMultiProcessorCount, a->device);
+  const uint64_t max_id = (a->h.state_len - 1) << a->h.stride2;
+  int end_bit = 1;
+  while (end_bit < 64 && (max_id >> end_bit)) ++end_bit;
+  if (ids) CK(cudaMemcpyAsync(w.d_soffs, ids, n_rows * 8, cudaMemcpyHostToDevice, w.stream));
+  CK(cudaEventRecord(w.ev0, w.stream));
+  CK(acb::launch_look_state(a->dev, p, w.stream));
+  if ((rc = cub_call(w, [&](void* t, size_t& tb) {
+         return acb::sort_pairs(t, tb, p.keys, p.skeys, p.rows, p.srows, n_rows, end_bit, w.stream);
+       })))
+    return rc;
+  CK(acb::launch_look_heads(p, w.stream));
+  if ((rc = cub_call(w, [&](void* t, size_t& tb) {
+         return acb::inclusive_sum_u64(t, tb, p.heads, p.heads, n_rows, w.stream);
+       })))
+    return rc;
+  CK(acb::launch_look_compact(p, w.stream));
+  CK(cudaEventRecord(w.ev1, w.stream));
+  CK(acb::launch_look_mask(a->dev, p, w.stream));
+  CK(cudaEventRecord(w.ev2, w.stream));
+  CK(acb::launch_look_copy(p, w.stream));
+  CK(cudaEventRecord(w.ev3, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, w.ev1, w.ev2);
+  w.stats.scan_ms = ms;
+  cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+  w.stats.order_ms = ms;
+  cudaEventElapsedTime(&ms, w.ev2, w.ev3);
+  w.stats.order_ms += ms;
+  w.stats.launches = 7;
+  if (dev_out) return ACG_OK;
+  CK(cudaEventRecord(w.ev0, w.stream));
+  if ((rc = copy_to_host(a, out, w.d_out, total))) return rc;
+  CK(cudaEventRecord(w.ev1, w.stream));
+  CK(cudaStreamSynchronize(w.stream));
+  cudaEventElapsedTime(&ms, w.ev0, w.ev1);
+  w.stats.d2h_ms = ms;
+  return ACG_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2839,6 +2934,65 @@ int acg_streams_flush(acg_streams* s, const uint64_t* ids, uint64_t n_ids, uint8
   }
   std::copy(offs.begin(), offs.end(), out_offsets);
   return ACG_OK;
+}
+
+int acg_candidates_create(const acg_dfa* a, const uint8_t* bytes, const uint64_t* offsets, uint64_t n_cands,
+                          acg_candidates** out) {
+  if (!a || !out || !offsets || n_cands >= (1ull << 32)) return ACG_E_INVALID_ARG;
+  *out = nullptr;
+  for (uint64_t i = 0; i < n_cands; ++i)
+    if (offsets[i + 1] < offsets[i]) return ACG_E_INVALID_ARG;
+  const uint64_t total = offsets[n_cands] - offsets[0];
+  if (total && !bytes) return ACG_E_INVALID_ARG;
+  if (!a->on_device) return ACG_E_NO_DEVICE;
+  std::vector<uint64_t> offs;
+  std::vector<uint8_t> cls;
+  try {
+    offs.resize(n_cands + 1);
+    cls.resize(total);
+  } catch (const std::bad_alloc&) {
+    return ACG_E_NOMEM;
+  }
+  for (uint64_t i = 0; i <= n_cands; ++i) offs[i] = offsets[i] - offsets[0];
+  for (uint64_t i = 0; i < total; ++i) cls[i] = a->h.classes[bytes[offsets[0] + i]];
+  acg_candidates* c = new (std::nothrow) acg_candidates();
+  if (!c) return ACG_E_NOMEM;
+  c->a = a;
+  c->n = n_cands;
+  DeviceGuard guard(a->device);
+  cudaError_t e = cudaMalloc(&c->d_offs, (n_cands + 1) * 8);
+  if (e != cudaSuccess) c->d_offs = nullptr;
+  if (e == cudaSuccess && (e = cudaMalloc(&c->d_classes, std::max<uint64_t>(total, 16))) != cudaSuccess)
+    c->d_classes = nullptr;
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_offs, offs.data(), (n_cands + 1) * 8, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && total) e = cudaMemcpy(c->d_classes, cls.data(), total, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    acg_candidates_free(c);
+    return e == cudaErrorMemoryAllocation ? ACG_E_NOMEM : ACG_E_CUDA;
+  }
+  *out = c;
+  return ACG_OK;
+}
+
+void acg_candidates_free(acg_candidates* c) {
+  if (!c) return;
+  {
+    DeviceGuard guard(c->a->device);
+    cudaFree(c->d_offs);
+    cudaFree(c->d_classes);
+  }
+  delete c;
+}
+
+int acg_streams_lookahead(const acg_streams* s, const acg_candidates* c, const uint64_t* ids, uint64_t n_ids,
+                          uint8_t* out) {
+  return streams_lookahead_impl(s, c, ids, n_ids, out, false);
+}
+
+int acg_streams_lookahead_devout(const acg_streams* s, const acg_candidates* c, const uint64_t* ids, uint64_t n_ids,
+                                 uint8_t* d_out) {
+  return streams_lookahead_impl(s, c, ids, n_ids, d_out, true);
 }
 
 int acg_find(const acg_dfa* a, const uint8_t* hay, uint64_t hay_len, uint64_t span_start,

@@ -301,6 +301,41 @@ cudaError_t launch_stream_hold(const StreamLaunch& p, cudaStream_t s);
 cudaError_t launch_stream_flush(const StreamLaunch& p, const uint64_t* ids, uint64_t n_ids,
                                 const uint64_t* out_offsets, uint8_t* out, cudaStream_t s);
 
+// Lookahead of a stream set (acg_streams_lookahead): for every row k (stream ids[k], or k when ids is nullptr) and
+// candidate c, out[k * n_cands + c] = 1 iff walking c from the state the row's stream tail leads to enters a match
+// state.  Steps:
+//   launch_look_state    thread k: the unanchored walk over its stream's tail (the StreamLaunch state), keys[k] =
+//                        that state id, rows[k] = k
+//   (sort_pairs on the state ids, end bit = the bits of the largest premultiplied id: skeys / srows)
+//   launch_look_heads    heads[i] = 1 where a run of equal states starts; an inclusive scan makes it the run index,
+//                        heads[n_rows - 1] = U, the number of distinct states, left in device memory
+//   launch_look_compact  run u gets its state ustate[u] and its first row urow[u]; every row its run, row_u[row]
+//   launch_look_mask     a persistent grid over U x ceil(n_cands / 32) warp items: lane c of item (u, g) walks candidate
+//                        32 g + c from ustate[u] and writes its byte in row urow[u]
+//   launch_look_copy     every other row copies its run's row, 4 KiB tiles, 16-byte stores where aligned
+// Indices into `out` are 64-bit.  n_rows < 2^32, n_cands < 2^32, n_rows * n_cands > 0.
+struct LookLaunch {
+  StreamLaunch st;                  // the set: n, back, pos, cursor, tail
+  const uint64_t* ids;              // [n_rows] or nullptr
+  uint64_t n_rows;
+  const uint64_t* cand_offsets;     // [n_cands + 1], from 0
+  const uint8_t* cand_classes;      // the candidates' bytes mapped through the automaton's byte classes
+  uint64_t n_cands;
+  uint64_t* keys;                   // [n_rows] state per row, then (after the sort) ustate[U]
+  uint32_t* rows;                   // [n_rows] row per entry, then urow[U]
+  uint64_t* skeys;                  // [n_rows] sorted states
+  uint32_t* srows;                  // [n_rows] their rows
+  unsigned long long* heads;        // [n_rows] run starts, then the run index (inclusive scan)
+  uint64_t* row_u;                  // [n_rows] the run of every row
+  uint8_t* out;                     // [n_rows * n_cands]
+  int sm_count;                     // the mask kernel's grid: a few CTAs per SM
+};
+cudaError_t launch_look_state(const DfaDev& dfa, const LookLaunch& p, cudaStream_t s);
+cudaError_t launch_look_heads(const LookLaunch& p, cudaStream_t s);
+cudaError_t launch_look_compact(const LookLaunch& p, cudaStream_t s);
+cudaError_t launch_look_mask(const DfaDev& dfa, const LookLaunch& p, cudaStream_t s);
+cudaError_t launch_look_copy(const LookLaunch& p, cudaStream_t s);
+
 // Offsets in device memory: result[0] = 1 if some offs[i] > offs[i + 1] or offs[n_docs] > hay_len (left as it
 // was otherwise: the caller clears it), result[1] = offs[0], result[2] = offs[n_docs].
 cudaError_t launch_check_offsets(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,

@@ -29,6 +29,11 @@
 //        stream_hold_kernel       a replace set's feed: the records of D with each stream's held bytes as a
 //                                 deletion after them, for the replace kernels to splice
 //        stream_flush_kernel      a replace set's flush: the listed streams' tails out, their state zeroed
+//        look_state_kernel        a stream set's lookahead: every row's state from its stream's tail, the
+//        look_heads_kernel        distinct states (after a sort) with one row each, the candidates walked
+//        look_compact_kernel      from every distinct state into that row, and the row copied to the rows
+//        look_mask_kernel         that share its state
+//        look_copy_kernel
 //        check_offsets_kernel     validation of document offsets in device memory
 //   K4  sort_pairs                ordering of the appended tuples (CUB radix sort)
 #include "acb_device.cuh"
@@ -825,6 +830,86 @@ __global__ void stream_flush_kernel(StreamLaunch p, const uint64_t* ids, uint64_
   }
 }
 
+// ---- lookahead of a stream set (LookLaunch) ----
+// Thread k: the state row k's stream is in, walked from the unanchored start over its tail.
+constexpr int kLookThreads = 256;
+__global__ void __launch_bounds__(kLookThreads) look_state_kernel(DfaDev d, LookLaunch p) {
+  __shared__ uint8_t s_cls[256];
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) s_cls[i] = d.classes[i];
+  __syncthreads();
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= p.n_rows) return;
+  const uint64_t s = p.ids ? p.ids[k] : k, len = stream_tail_len(p.st, s);
+  const uint8_t* tail = p.st.tail + s * p.st.back;
+  uint32_t sid = d.start_unanchored_id;
+  for (uint64_t j = 0; j < len; ++j) sid = __ldg(d.trans + sid + s_cls[tail[j]]);
+  p.keys[k] = sid;
+  p.rows[k] = (uint32_t)k;
+}
+
+__global__ void look_heads_kernel(LookLaunch p) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < p.n_rows) p.heads[i] = i == 0 || p.skeys[i] != p.skeys[i - 1];
+}
+
+// After the scan heads[i] is 1 + the run of entry i: the head of run u stores its state and row, every entry its run.
+__global__ void look_compact_kernel(LookLaunch p) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.n_rows) return;
+  const uint64_t u = p.heads[i] - 1;
+  const uint32_t row = p.srows[i];
+  p.row_u[row] = u;
+  if (i == 0 || p.heads[i - 1] != p.heads[i]) {
+    p.keys[u] = p.skeys[i];
+    p.rows[u] = row;
+  }
+}
+
+// Warp item (u, g), items in that order so that neighbouring warps share a state: lane c walks candidate 32 g + c
+// from state keys[u] and stops at the first match state (DEAD ends the walk without one).  The candidates' bytes are
+// class ids already.  U is read here, so the grid does not depend on it.
+__global__ void __launch_bounds__(kLookThreads) look_mask_kernel(DfaDev d, LookLaunch p) {
+  const uint64_t n_u = p.heads[p.n_rows - 1], groups = (p.n_cands + 31) >> 5, items = n_u * groups;
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  const uint32_t* __restrict__ trans = d.trans;
+  const uint32_t max_match = d.max_match_id;
+  for (uint64_t it = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; it < items; it += warps) {
+    const uint64_t u = it / groups, c = (it - u * groups) * 32 + lane;
+    if (c >= p.n_cands) continue;
+    uint32_t sid = (uint32_t)p.keys[u];
+    uint8_t hit = 0;
+    const uint64_t hi = __ldg(p.cand_offsets + c + 1);
+    for (uint64_t q = __ldg(p.cand_offsets + c); q < hi; ++q) {
+      sid = __ldg(trans + sid + __ldg(p.cand_classes + q));
+      if (sid <= max_match) {
+        hit = sid != 0;
+        break;
+      }
+    }
+    p.out[(uint64_t)p.rows[u] * p.n_cands + c] = hit;
+  }
+}
+
+// Item (row, tile): a row whose run is written by another row copies that row's tile of kSpliceTile bytes, one
+// 16-byte piece per thread.
+__global__ void __launch_bounds__(kSpliceThreads) look_copy_kernel(LookLaunch p) {
+  const uint64_t tiles = (p.n_cands + kSpliceTile - 1) / kSpliceTile;
+  for (uint64_t it = blockIdx.x; it < p.n_rows * tiles; it += gridDim.x) {
+    const uint64_t k = it / tiles, o = (it - k * tiles) * kSpliceTile + threadIdx.x * 16;
+    const uint64_t r = p.rows[p.row_u[k]];
+    if (r == k || o >= p.n_cands) continue;
+    const uint8_t* src = p.out + r * p.n_cands + o;
+    uint8_t* dst = p.out + k * p.n_cands + o;
+    const uint64_t n = p.n_cands - o < 16 ? p.n_cands - o : 16;
+    if (n == 16 && !((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15)) {
+      *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
+    } else {
+      for (uint64_t j = 0; j < n; ++j) dst[j] = src[j];
+    }
+  }
+}
+
 __global__ void check_offsets_kernel(const uint64_t* offs, uint64_t n_docs, uint64_t hay_len,
                                      unsigned long long* result) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1036,6 +1121,36 @@ cudaError_t launch_stream_hold(const StreamLaunch& p, cudaStream_t s) {
 cudaError_t launch_stream_flush(const StreamLaunch& p, const uint64_t* ids, uint64_t n_ids,
                                 const uint64_t* out_offsets, uint8_t* out, cudaStream_t s) {
   ACB_LAUNCH(stream_flush_kernel, (unsigned)((n_ids * 32 + 255) / 256), 256, 0, s, p, ids, n_ids, out_offsets, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_look_state(const DfaDev& dfa, const LookLaunch& p, cudaStream_t s) {
+  ACB_LAUNCH(look_state_kernel, (unsigned)((p.n_rows + kLookThreads - 1) / kLookThreads), kLookThreads, 0, s, dfa, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_look_heads(const LookLaunch& p, cudaStream_t s) {
+  ACB_LAUNCH(look_heads_kernel, (unsigned)((p.n_rows + 255) / 256), 256, 0, s, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_look_compact(const LookLaunch& p, cudaStream_t s) {
+  ACB_LAUNCH(look_compact_kernel, (unsigned)((p.n_rows + 255) / 256), 256, 0, s, p);
+  return cudaGetLastError();
+}
+
+// Eight CTAs of 256 threads fill an SM; no more warps than the largest U (n_rows) could use.
+cudaError_t launch_look_mask(const DfaDev& dfa, const LookLaunch& p, cudaStream_t s) {
+  const uint64_t warps = p.n_rows * ((p.n_cands + 31) >> 5), per_cta = kLookThreads / 32;
+  const uint64_t grid = std::min<uint64_t>((uint64_t)p.sm_count * 8, (warps + per_cta - 1) / per_cta);
+  ACB_LAUNCH(look_mask_kernel, (unsigned)grid, kLookThreads, 0, s, dfa, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_look_copy(const LookLaunch& p, cudaStream_t s) {
+  const uint64_t items = p.n_rows * ((p.n_cands + kSpliceTile - 1) / kSpliceTile);
+  const uint64_t grid = std::min<uint64_t>((uint64_t)p.sm_count * 8, items);
+  ACB_LAUNCH(look_copy_kernel, (unsigned)grid, kSpliceThreads, 0, s, p);
   return cudaGetLastError();
 }
 

@@ -424,6 +424,38 @@ int acg_streams_flush(acg_streams* set, const uint64_t* ids, uint64_t n_ids, uin
                       uint64_t* out_offsets, uint64_t* out_len);
 int acg_streams_held(const acg_streams* set, uint64_t* held);
 
+/* ---- lookahead: which of a fixed set of candidate chunks would complete a match ------------
+ * A candidate set is a fixed list of byte strings (a tokenizer's vocabulary, say), uploaded once
+ * and reused by every call: candidate i is bytes[offsets[i] .. offsets[i + 1]).
+ * acg_candidates_create: n_cands >= 2^32, decreasing offsets, a NULL offsets or out, or a NULL
+ * bytes with bytes to copy give ACG_E_INVALID_ARG; ACG_E_NOMEM when they do not fit.  The
+ * candidates are copied to the automaton's device, mapped through its byte classes, so the set is
+ * bound to that automaton, which must outlive it; the caller's arrays are not kept.
+ * acg_streams_lookahead(_devout): for a stream or replace set whose stream s has received X_s
+ * (pos_s = |X_s|), row k of the output is stream ids[k] (ids == NULL: n_streams rows, row k is
+ * stream k; ids in host memory, duplicates and any order allowed), and
+ *   out[k * n_cands + c] = 1 iff a feed that gave that stream candidate c as its chunk would
+ *   return at least one match for it: the set's iterator (find_iter with its restart point, or
+ *   overlapping; find_iter for a replace set) over X_s | c has a match whose end lies in
+ *   (pos_s, pos_s + |c|]; else 0.
+ * Empty candidates never match, so a caller whose logits are wider than its vocabulary pads the
+ * list with empty candidates.  out holds n_rows * n_cands bytes, row-major, 0 or 1 each: host memory
+ * for acg_streams_lookahead, device memory for _devout.  The call reads the streams and changes
+ * none of them.  A candidate set from another automaton, a NULL set or candidate set, an id
+ * >= n_streams, n_ids >= 2^32 or a NULL out with n_rows * n_cands > 0 give ACG_E_INVALID_ARG and
+ * write nothing; a workspace that cannot grow gives ACG_E_NOMEM.  One call at a time per stream
+ * set, as for feeds; a candidate set may be shared by concurrent calls on different sets.
+ * acg_last_stats: the mask kernel in scan_ms, the rest of the device work (the rows' states, their
+ * dedupe and the copy of shared rows) in order_ms. */
+typedef struct acg_candidates acg_candidates;
+int acg_candidates_create(const acg_dfa* dfa, const uint8_t* bytes, const uint64_t* offsets, uint64_t n_cands,
+                          acg_candidates** out);
+void acg_candidates_free(acg_candidates* cands);
+int acg_streams_lookahead(const acg_streams* set, const acg_candidates* cands, const uint64_t* ids, uint64_t n_ids,
+                          uint8_t* out);
+int acg_streams_lookahead_devout(const acg_streams* set, const acg_candidates* cands, const uint64_t* ids,
+                                 uint64_t n_ids, uint8_t* d_out);
+
 /* ---- multi-GPU: haystack slices + gather of match buffers to rank 0 (SURVEY.md section 8e) ----
  * One process (or thread) per GPU.  The path shards naturally: rank g owns the matches whose END
  * lies in (own_lo, own_hi] (rank 0 also owns end == span_start: empty-pattern matches of the start

@@ -546,6 +546,57 @@ class AhoCorasick {
   mutable uint64_t cap_hint_ = 4096;
 };
 
+// A candidate set (acg_candidates_create, include/acb200.h): a fixed list of byte strings -- a tokenizer's vocabulary,
+// say -- on the automaton's device, for the lookahead of that automaton's stream sets.  The automaton must outlive it.
+class Candidates {
+ public:
+  template <class Strings>
+  Candidates(const AhoCorasick& ac, const Strings& cands) {
+    std::string bytes;
+    std::vector<uint64_t> at{0};
+    for (const auto& x : cands) {
+      bytes.append(std::string_view(x));
+      at.push_back(bytes.size());
+    }
+    Result<int> r;
+    r.error = acg_candidates_create(ac.raw(), reinterpret_cast<const uint8_t*>(bytes.data()), at.data(),
+                                    at.size() - 1, &h_);
+    r.unwrap();
+    n_ = at.size() - 1;
+  }
+  Candidates(Candidates&& o) noexcept : h_(o.h_), n_(o.n_) { o.h_ = nullptr; }
+  Candidates& operator=(Candidates&& o) noexcept {
+    if (this != &o) { close(); h_ = o.h_; n_ = o.n_; o.h_ = nullptr; }
+    return *this;
+  }
+  Candidates(const Candidates&) = delete;
+  Candidates& operator=(const Candidates&) = delete;
+  ~Candidates() { close(); }
+
+  uint64_t size() const { return n_; }
+  acg_candidates* raw() const { return h_; }
+
+ private:
+  void close() {
+    if (h_) acg_candidates_free(h_);
+    h_ = nullptr;
+  }
+  acg_candidates* h_ = nullptr;
+  uint64_t n_ = 0;
+};
+
+namespace detail {
+// acg_streams_lookahead: rows(ids) x cands.size() bytes, row-major, 1 where feeding that row's stream that candidate
+// would return a match.  An empty `ids` takes every one of the set's n streams.
+inline Result<std::vector<uint8_t>> lookahead(const acg_streams* set, uint64_t n, const Candidates& cands,
+                                              const std::vector<uint64_t>& ids) {
+  Result<std::vector<uint8_t>> r;
+  r.value.resize((ids.empty() ? n : ids.size()) * cands.size());
+  r.error = acg_streams_lookahead(set, cands.raw(), ids.empty() ? nullptr : ids.data(), ids.size(), r.value.data());
+  return r;
+}
+}  // namespace detail
+
 // A stream set (acg_streams_*, include/acb200.h): n streams searched on the device as their bytes arrive.  feed()
 // takes one chunk per stream -- CSR `offsets` [n + 1] into `chunks` -- and returns, per stream, the matches of the
 // mode's iterator (find_iter, or find_overlapping_iter when `overlapping`) over all the stream's bytes that end in
@@ -614,6 +665,14 @@ class Streams {
     r.error = acg_streams_positions(h_, pos.data());
     r.unwrap();
     return pos;
+  }
+  // For every row -- stream ids[k], or every stream when ids is empty -- and every candidate c: 1 if feeding that
+  // stream c would return a match, row-major.  No stream changes.
+  Result<std::vector<uint8_t>> try_lookahead(const Candidates& cands, const std::vector<uint64_t>& ids = {}) const {
+    return detail::lookahead(h_, n_, cands, ids);
+  }
+  std::vector<uint8_t> lookahead(const Candidates& cands, const std::vector<uint64_t>& ids = {}) const {
+    return std::move(try_lookahead(cands, ids).unwrap());
   }
   acg_streams* raw() const { return h_; }
 
@@ -710,6 +769,13 @@ class ReplaceStreams {
     r.error = acg_streams_held(h_, h.data());
     r.unwrap();
     return h;
+  }
+  // As Streams::lookahead: 1 where feeding the row's stream the candidate would replace a match.
+  Result<std::vector<uint8_t>> try_lookahead(const Candidates& cands, const std::vector<uint64_t>& ids = {}) const {
+    return detail::lookahead(h_, n_, cands, ids);
+  }
+  std::vector<uint8_t> lookahead(const Candidates& cands, const std::vector<uint64_t>& ids = {}) const {
+    return std::move(try_lookahead(cands, ids).unwrap());
   }
   acg_streams* raw() const { return h_; }
 
